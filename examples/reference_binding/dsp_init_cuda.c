@@ -27,6 +27,7 @@
 /* ---- prototypes of include/avdsp_b200.h, repeated so that the reference's struct definitions are the ones in scope ---- */
 int  avb200_init(int device);
 void ff_idctdsp_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample, unsigned high_bit_depth);
+void ff_xvid_idct_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample);
 void ff_fdctdsp_init_cuda(FDCTDSPContext *c, int dct_algo, int bits_per_raw_sample, unsigned high_bit_depth);
 void ff_blockdsp_init_cuda(BlockDSPContext *c);
 void ff_me_cmp_init_cuda(MECmpContext *c);
@@ -71,6 +72,11 @@ void ff_idctdsp_init_cuda_hook(IDCTDSPContext *c, AVCodecContext *avctx, unsigne
 {
     ff_idctdsp_init_cuda(c, avctx->idct_algo, avctx->bits_per_raw_sample, high_bit_depth);
 }
+/* mpeg4videodec.c:2084-2085 and :2558-2559, right after each ff_xvid_idct_init(&s->idsp, avctx) */
+void ff_xvid_idct_init_cuda_hook(IDCTDSPContext *c, AVCodecContext *avctx)
+{
+    ff_xvid_idct_init_cuda(c, avctx->idct_algo, avctx->bits_per_raw_sample);
+}
 void ff_fdctdsp_init_cuda_hook(FDCTDSPContext *c, AVCodecContext *avctx, unsigned high_bit_depth)      /* fdctdsp.c:45-48 */
 {
     ff_fdctdsp_init_cuda(c, avctx->dct_algo, avctx->bits_per_raw_sample, high_bit_depth);
@@ -89,6 +95,7 @@ void all_hooks_take_the_reference_types(IDCTDSPContext *a, FDCTDSPContext *b, Bl
                                         PixblockDSPContext *j, QpelDSPContext *k, FFTContext *l, AVCodecContext *avctx)
 {
     ff_idctdsp_init_cuda_hook(a, avctx, avctx->bits_per_raw_sample > 8);
+    ff_xvid_idct_init_cuda_hook(a, avctx);
     ff_fdctdsp_init_cuda_hook(b, avctx, avctx->bits_per_raw_sample > 8);
     ff_blockdsp_init_cuda(c);
     ff_me_cmp_init_cuda(d);

@@ -86,6 +86,14 @@ int ff_pixels_clamped_batch_cuda(int mode, const int16_t *blocks, uint8_t *frame
  * functions leave them.  Functional path for 10-bit content (thread per block), not tuned like the 8-bit kernel. */
 int ff_simple_idct10_batch_cuda(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, void *stream);
 
+/* ff_xvid_idct / xvid_idct_put / xvid_idct_add (libavcodec/xvididct.c:272-331) over n blocks -- the IDCT ff_xvid_idct_init() installs for
+ * MPEG-4 streams written by Xvid and for idct_algo FF_IDCT_XVID.  Arguments, addressing, mode 0 / 1 / 2 and `clear` exactly as
+ * ff_simple_idct_batch_cuda; mode 2 leaves the transform result in the blocks.  Blocks at any 2-byte alignment and destinations at any
+ * byte alignment are accepted: a batch whose blocks are not 16-byte aligned, or whose frame or stride is not a multiple of 8, runs a
+ * thread-per-block kernel instead of the staged one (with dst_off, the offsets must then keep 8-byte alignment as well). */
+int ff_xvid_idct_batch_cuda(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
+                            size_t n, int tiles_per_row, int clear, void *stream);
+
 /* BlockDSPContext.clear_block / clear_blocks over n_blocks * 64 coefficients (blockdsp.c:29-37) and
  * fill_block_tab[w16 ? 0 : 1] over n records (blockdsp.c:39-58). */
 int ff_clear_blocks_batch_cuda(int16_t *blocks, size_t n_blocks, void *stream);
@@ -132,6 +140,13 @@ int ff_mpeg_dequant_batch_cuda(int kind, const FFMpegDequantTables *tables, cons
 int ff_mpeg_dequant_idct_batch_cuda(int kind, const FFMpegDequantTables *tables, const FFMpegDequantBlock *recs, int16_t *blocks,
                                     uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row,
                                     int clear, void *stream);
+
+/* put_dct / add_dequant_dct (mpegvideo.c:1401-1427) with the Xvid IDCT: same arguments, kinds and skipping rules as
+ * ff_mpeg_dequant_idct_batch_cuda, the transform of ff_xvid_idct_batch_cuda.  Blocks must be 16-byte aligned, frame and stride multiples
+ * of 8 (and dst_off entries too); anything else is refused. */
+int ff_mpeg_dequant_xvid_idct_batch_cuda(int kind, const FFMpegDequantTables *tables, const FFMpegDequantBlock *recs, int16_t *blocks,
+                                         uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row,
+                                         int clear, void *stream);
 
 /* Residual: H264DSPContext.h264_idct_add16 / _add16intra / idct8_add4 (+ h264_idct_add8 for chroma)
  * (libavcodec/h264idct_template.c:174-214).  Record i consumes coeffs + i * coeff_stride (int16; block k of the MB at
@@ -520,6 +535,10 @@ int  sws_debug_slot_view_cuda(int srcW, int srcH, int srcFormat, int dstW, int d
  * Taken over: idct_algo FF_IDCT_SIMPLE / FF_IDCT_AUTO at 8 bit, and bits_per_raw_sample 10 (ff_simple_idct_*_10 whatever idct_algo says,
  * idctdsp.c:151-155); anything else leaves `c` untouched. */
 void ff_idctdsp_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample, unsigned high_bit_depth);
+/* The arch hook of ff_xvid_idct_init (libavcodec/xvididct.c:333-350), called after it: idct / idct_put / idct_add, perm_type =
+ * FF_IDCT_PERM_NONE and an identity idct_permutation when bits_per_raw_sample <= 8 and idct_algo is FF_IDCT_AUTO or FF_IDCT_XVID
+ * (AVB_FF_IDCT_XVID); otherwise `c` is untouched.  ff_idctdsp_init_cuda leaves FF_IDCT_XVID alone, like the reference's ff_idctdsp_init. */
+void ff_xvid_idct_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample);
 void ff_blockdsp_init_cuda(BlockDSPContext *c);   /* libavcodec/blockdsp.c:60-74 */
 /* libavcodec/fdctdsp.c:27-50 (same shape as ff_fdctdsp_init_x86): dct_algo FF_DCT_AUTO / FF_DCT_INT -> islow,
  * FF_DCT_FASTINT -> ifast; bits_per_raw_sample 10 -> jpeg_fdct_islow_10 / fdct248_islow_10; FF_DCT_FAAN is left to the C path */

@@ -37,6 +37,7 @@ typedef struct IDCTDSPContext {
 /* idct_algo values the hook understands (libavcodec/avcodec.h FF_IDCT_*) */
 #define AVB_FF_IDCT_AUTO   0
 #define AVB_FF_IDCT_SIMPLE 2
+#define AVB_FF_IDCT_XVID   14
 
 /* ---- libavcodec/fdctdsp.h:26-29 ---- */
 typedef struct FDCTDSPContext {

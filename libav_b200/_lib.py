@@ -58,6 +58,7 @@ PROTOTYPES = {
     "avb200_event_elapsed_ms": (C.c_float, [vp, vp]),
     "ff_simple_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_simple_idct10_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, vp]),
+    "ff_xvid_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_pixels_clamped_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, vp]),
     "ff_clear_blocks_batch_cuda": (i32, [vp, sz, vp]),
     "ff_fill_blocks_batch_cuda": (i32, [vp, vp, vp, pd, i32, i32, sz, vp]),
@@ -76,6 +77,7 @@ PROTOTYPES = {
     "ff_pixblock_fdct_batch_cuda": (i32, [i32, vp, vp, vp, vp, pd, vp, sz, vp]),
     "ff_mpeg_dequant_batch_cuda": (i32, [i32, vp, vp, vp, sz, vp]),
     "ff_mpeg_dequant_idct_batch_cuda": (i32, [i32, vp, vp, vp, vp, vp, pd, sz, i32, i32, vp]),
+    "ff_mpeg_dequant_xvid_idct_batch_cuda": (i32, [i32, vp, vp, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_me_cmp_batch_cuda": (i32, [i32, i32, i32, vp, vp, pd, i32, vp, sz, vp, vp]),
     "ff_h264_idct_add_mb_batch_hbd_cuda": (i32, [i32, i32, vp, sz, vp, sz, vp, vp, vp, vp, i32, i32, vp]),
     "ff_h264_mc_batch_hbd_cuda": (i32, [i32, i32, vp, sz, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -105,6 +107,7 @@ PROTOTYPES = {
     "sws_debug_plan_cuda": (i32, [i32, i32, i32, i32, i32, i32, i32, vp]),
     "sws_debug_slot_view_cuda": (i32, [i32, i32, i32, i32, i32, i32, i32, vp]),
     "ff_idctdsp_init_cuda": (None, [vp, i32, i32, C.c_uint]),
+    "ff_xvid_idct_init_cuda": (None, [vp, i32, i32]),
     "ff_blockdsp_init_cuda": (None, [vp]),
     "ff_fdctdsp_init_cuda": (None, [vp, i32, i32, C.c_uint]),
     "ff_me_cmp_init_cuda": (None, [vp]),

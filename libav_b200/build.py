@@ -4,6 +4,7 @@
   oracle/liboracle_port.so      TEST ONLY: plain-C restatement of the reference path (gcc)
   oracle/_ref/libavref.so       TEST ONLY: the unmodified reference compiled from /root/reference,
                                 only when that tree is present (never on the GPU box)
+  oracle/_ref/libxvidref.so     TEST ONLY: the reference's Xvid IDCT, same conditions
 All outputs are in-tree so they travel to the GPU box with the snapshot.
 """
 import glob
@@ -82,6 +83,8 @@ def build_oracle_ref(force=False):
     if force:
         shutil.rmtree(os.path.join(ROOT, "oracle", "_ref"), ignore_errors=True)
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "REF=" + REFERENCE])
+    # the Xvid IDCT (oracle/_ref/libxvidref.so), linked against libavref.so
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "xvid.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

@@ -15,6 +15,8 @@ int launch_clear_blocks(int16_t *blocks, size_t n_blocks, cudaStream_t st);
 int launch_mpeg_dequant(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, size_t n, cudaStream_t st);
 int launch_mpeg_dequant_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
                              const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st);
+int launch_mpeg_dequant_xvid_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
+                                  const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st);
 int launch_fill_blocks(uint8_t *frame, const uint32_t *dst_off, const uint8_t *value, ptrdiff_t stride, int h,
                        int w16, size_t n, cudaStream_t st);
 }
@@ -64,6 +66,20 @@ int ff_mpeg_dequant_idct_batch_cuda(int kind, const FFMpegDequantTables *t, cons
     if (dq_tables("ff_mpeg_dequant_idct_batch_cuda", kind, t, d)) return -1;
     return launch_mpeg_dequant_idct(kind, d, reinterpret_cast<const uint32_t *>(recs), blocks, frame, dst_off, stride, n, tiles_per_row,
                                     clear, (cudaStream_t)stream);
+}
+int ff_mpeg_dequant_xvid_idct_batch_cuda(int kind, const FFMpegDequantTables *t, const FFMpegDequantBlock *recs, int16_t *blocks,
+                                         uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row,
+                                         int clear, void *stream)
+{
+    avb::enter();
+    DqTables d;
+    if (dq_tables("ff_mpeg_dequant_xvid_idct_batch_cuda", kind, t, d)) return -1;
+    if (n && (((uintptr_t)blocks & 15) || (((uintptr_t)frame | (uintptr_t)stride) & 7))) {
+        set_error_msg("ff_mpeg_dequant_xvid_idct_batch_cuda", "blocks must be 16-byte aligned, frame and stride multiples of 8");
+        return -1;
+    }
+    return launch_mpeg_dequant_xvid_idct(kind, d, reinterpret_cast<const uint32_t *>(recs), blocks, frame, dst_off, stride, n, tiles_per_row,
+                                         clear, (cudaStream_t)stream);
 }
 int ff_clear_blocks_batch_cuda(int16_t *blocks, size_t n_blocks, void *stream)
 {

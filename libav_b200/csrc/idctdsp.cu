@@ -15,10 +15,13 @@
 //     writes 256 contiguous bytes per picture row.
 // Two tiles per warp are double-buffered so the next group's loads fly during the math.
 // Algorithmic traffic: put 128 B in + 64 B out (+4 B offset) per block; add 256 B; idct 256 B.
+// The two passes are a policy of the kernel template (SimpleIdct here, XvidIdct in xvid_idct.cuh for ff_xvid_idct): everything else
+// -- staging, fetch, addressing, fused clear and dequantisation -- is shared.
 #include "common.cuh"
 #include <type_traits>
 #include <cuda.h>            // CUtensorMap only; the encoder is looked up at run time (no libcuda link dependency)
 #include "idct_dq.h"
+#include "xvid_idct.cuh"
 
 namespace avb {
 
@@ -83,6 +86,12 @@ __device__ __forceinline__ void col_pass(const uint32_t (&w)[8], int (&out)[8])
 #pragma unroll
     for (int k = 0; k < 4; k++) { out[k] = sra<20, MH>(s[k]); out[7 - k] = sra<20, MH>(d[k]); }
 }
+
+// the transform policy of simple_idct_kernel: this file's simple IDCT (xvid_idct.cuh has the Xvid one)
+struct SimpleIdct {
+    template <bool MH> static __device__ __forceinline__ uint4 row(uint4 v, int) { return row_pass<MH>(v); }
+    template <int HI, bool MH> static __device__ __forceinline__ void col(const uint32_t (&w)[8], int (&out)[8]) { col_pass<HI, MH>(w, out); }
+};
 
 __device__ __forceinline__ size_t block_dst(const uint32_t *__restrict__ dst_off, size_t i,
                                             int tiles_per_row, ptrdiff_t stride)
@@ -182,7 +191,8 @@ struct NoTma {};
 // TMA: the warp's 4 KB group arrives by ONE cp.async.bulk.tensor issued by lane 0 (2-D tensor map over the block array,
 // box 32 blocks x 128 B, SWIZZLE_128B = the same chunk ^ (block & 7) layout the cp.async path builds by hand) and is
 // awaited on an mbarrier, instead of eight cp.async per lane.
-template <int MODE, bool CLEAR, int MINB = 5, bool MH = false, int DQ = 0, bool TMA = false>
+// XF: the transform (SimpleIdct, XvidIdct): its row pass on each packed row and its column pass; everything else is shared.
+template <int MODE, bool CLEAR, int MINB = 5, bool MH = false, int DQ = 0, bool TMA = false, class XF = SimpleIdct>
 __global__ void __launch_bounds__(IDCT_WARPS * 32, MINB)
 simple_idct_kernel(int16_t *__restrict__ blocks, uint8_t *__restrict__ frame,
                    const uint32_t *__restrict__ dst_off, ptrdiff_t stride, size_t n, int tiles_per_row,
@@ -270,10 +280,10 @@ simple_idct_kernel(int16_t *__restrict__ blocks, uint8_t *__restrict__ frame,
             int sum = -1;
 #pragma unroll
             for (int r = 0; r < 8; r++)
-                row[r] = row_pass<MH>(dq_row<DQ - 1>(lds128(tb + rd_base + (((unsigned)r << 4) ^ rd_key)), r, dq.t, L, sum));
+                row[r] = XF::template row<MH>(dq_row<DQ - 1>(lds128(tb + rd_base + (((unsigned)r << 4) ^ rd_key)), r, dq.t, L, sum), r);
         } else {
 #pragma unroll
-            for (int r = 0; r < 8; r++) row[r] = row_pass<MH>(lds128(tb + rd_base + (((unsigned)r << 4) ^ rd_key)));
+            for (int r = 0; r < 8; r++) row[r] = XF::template row<MH>(lds128(tb + rd_base + (((unsigned)r << 4) ^ rd_key)), r);
         }
         __syncwarp();     // this buffer is free for the load issued two iterations from now
 
@@ -286,8 +296,8 @@ simple_idct_kernel(int16_t *__restrict__ blocks, uint8_t *__restrict__ frame,
 #pragma unroll
                 for (int r = 0; r < 8; r++) w[r] = c == 0 ? row[r].x : c == 1 ? row[r].y : c == 2 ? row[r].z : row[r].w;
                 int lo[8], hi[8];
-                col_pass<0, MH>(w, lo);
-                col_pass<1, MH>(w, hi);
+                XF::template col<0, MH>(w, lo);
+                XF::template col<1, MH>(w, hi);
 #pragma unroll
                 for (int y = 0; y < 8; y++) o[y][c] = pack16(lo[y], hi[y]);
             }
@@ -319,8 +329,8 @@ simple_idct_kernel(int16_t *__restrict__ blocks, uint8_t *__restrict__ frame,
 #pragma unroll
                     for (int r = 0; r < 8; r++)
                         w[r] = h == 0 ? (c == 0 ? row[r].x : row[r].y) : (c == 0 ? row[r].z : row[r].w);
-                    col_pass<0, MH>(w, v[2 * c]);
-                    col_pass<1, MH>(w, v[2 * c + 1]);
+                    XF::template col<0, MH>(w, v[2 * c]);
+                    XF::template col<1, MH>(w, v[2 * c + 1]);
                 }
 #pragma unroll
                 for (int y = 0; y < 8; y++) {
@@ -425,12 +435,14 @@ static bool make_block_tensor_map(CUtensorMap *tm, const int16_t *blocks, size_t
               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-int launch_simple_idct(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
-                       size_t n, int tiles_per_row, int clear, cudaStream_t st)
+// the staged 8-bit IDCT with transform XF over n blocks; `who` names the entry point in error messages
+template <class XF>
+static int launch_idct8(const char *who, int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
+                        size_t n, int tiles_per_row, int clear, cudaStream_t st)
 {
     if (n == 0) return 0;
-    if (mode < 0 || mode > 2) { set_error_msg("simple_idct_batch", "bad mode"); return -1; }
-    if (mode != 2 && !dst_off && tiles_per_row <= 0) { set_error_msg("simple_idct_batch", "need dst_off or tiles_per_row"); return -1; }
+    if (mode < 0 || mode > 2) { set_error_msg(who, "bad mode"); return -1; }
+    if (mode != 2 && !dst_off && tiles_per_row <= 0) { set_error_msg(who, "need dst_off or tiles_per_row"); return -1; }
     size_t groups = (n + 31) / 32;
     // 16 CTAs per SM in the grid (about 3 waves of the 5 resident ones) rather than exactly one persistent wave: the shorter per-CTA
     // loops even out the tail
@@ -441,20 +453,33 @@ int launch_simple_idct(int mode, int16_t *blocks, uint8_t *frame, const uint32_t
     if (mode == 0 && !clear && tuning("idct_tma") != 2 && !((uintptr_t)blocks & 15)) {
         CUtensorMap tm;
         if (make_block_tensor_map(&tm, blocks, n)) {
-            simple_idct_kernel<0, false, 5, false, 0, true><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, NoDq{}, tm);
-            return check_launch("simple_idct_batch");
+            simple_idct_kernel<0, false, 5, false, 0, true, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, NoDq{}, tm);
+            return check_launch(who);
         }
     }
     if (mode == 0) {
-        if (clear) simple_idct_kernel<0, true><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
-        else       simple_idct_kernel<0, false><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        if (clear) simple_idct_kernel<0, true, 5, false, 0, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        else       simple_idct_kernel<0, false, 5, false, 0, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
     } else if (mode == 1) {
-        if (clear) simple_idct_kernel<1, true><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
-        else       simple_idct_kernel<1, false><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        if (clear) simple_idct_kernel<1, true, 5, false, 0, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        else       simple_idct_kernel<1, false, 5, false, 0, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
     } else {
-        simple_idct_kernel<2, false><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        simple_idct_kernel<2, false, 5, false, 0, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
     }
-    return check_launch("simple_idct_batch");
+    return check_launch(who);
+}
+
+int launch_simple_idct(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
+                       size_t n, int tiles_per_row, int clear, cudaStream_t st)
+{
+    return launch_idct8<SimpleIdct>("simple_idct_batch", mode, blocks, frame, dst_off, stride, n, tiles_per_row, clear, st);
+}
+
+// the Xvid IDCT through the same kernel: 16-byte aligned blocks and, for put / add, 8-byte aligned destinations (xvid_idct.cu decides)
+int launch_xvid_idct_staged(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
+                            size_t n, int tiles_per_row, int clear, cudaStream_t st)
+{
+    return launch_idct8<XvidIdct>("xvid_idct_batch", mode, blocks, frame, dst_off, stride, n, tiles_per_row, clear, st);
 }
 
 template <int KIND>
@@ -490,24 +515,37 @@ int launch_mpeg_dequant(int kind, const DqTables &t, const uint32_t *recs, int16
 }
 
 // intra kinds run as idct_put, inter kinds as idct_add (put_dct / add_dequant_dct, libavcodec/mpegvideo.c:1401-1427)
-int launch_mpeg_dequant_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
-                             const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st)
+template <class XF>
+static int launch_dequant_idct8(const char *who, int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
+                                const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st)
 {
     if (n == 0) return 0;
-    if (!dst_off && tiles_per_row <= 0) { set_error_msg("mpeg_dequant_idct_batch", "need dst_off or tiles_per_row"); return -1; }
+    if (!dst_off && tiles_per_row <= 0) { set_error_msg(who, "need dst_off or tiles_per_row"); return -1; }
     const size_t groups = (n + 31) / 32;
     const int grid = grid_for(groups, IDCT_WARPS, 16);
     const dim3 b(IDCT_WARPS * 32);
     DqArgs a; a.recs = recs; a.t = t;
 #define AVB_DQ(K, MODE) \
-    case K: if (clear) simple_idct_kernel<MODE, true, 4, false, K + 1><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, a); \
-            else       simple_idct_kernel<MODE, false, 4, false, K + 1><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, a); break;
+    case K: if (clear) simple_idct_kernel<MODE, true, 4, false, K + 1, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, a); \
+            else       simple_idct_kernel<MODE, false, 4, false, K + 1, false, XF><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, a); break;
     switch (kind) {
     AVB_DQ(0, 0) AVB_DQ(1, 1) AVB_DQ(2, 0) AVB_DQ(3, 0) AVB_DQ(4, 1) AVB_DQ(5, 0) AVB_DQ(6, 1)
-    default: set_error_msg("mpeg_dequant_idct_batch", "bad kind"); return -1;
+    default: set_error_msg(who, "bad kind"); return -1;
     }
 #undef AVB_DQ
-    return check_launch("mpeg_dequant_idct_batch");
+    return check_launch(who);
+}
+
+int launch_mpeg_dequant_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
+                             const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st)
+{
+    return launch_dequant_idct8<SimpleIdct>("mpeg_dequant_idct_batch", kind, t, recs, blocks, frame, dst_off, stride, n, tiles_per_row, clear, st);
+}
+
+int launch_mpeg_dequant_xvid_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
+                                  const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st)
+{
+    return launch_dequant_idct8<XvidIdct>("mpeg_dequant_xvid_idct_batch", kind, t, recs, blocks, frame, dst_off, stride, n, tiles_per_row, clear, st);
 }
 
 int launch_pixels_clamped(int mode, const int16_t *blocks, uint8_t *frame, const uint32_t *dst_off,

@@ -4,7 +4,7 @@ import ctypes as C
 
 u8p, i16p, i8p = C.POINTER(C.c_uint8), C.POINTER(C.c_int16), C.POINTER(C.c_int8)
 pd = C.c_ssize_t
-FF_IDCT_AUTO, FF_IDCT_SIMPLE = 0, 2
+FF_IDCT_AUTO, FF_IDCT_SIMPLE, FF_IDCT_XVID = 0, 2, 14
 
 _clamped = C.CFUNCTYPE(None, i16p, u8p, pd)
 _idct = C.CFUNCTYPE(None, i16p)
