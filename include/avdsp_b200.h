@@ -449,6 +449,87 @@ int ff_hpel_batch_cuda(const FFHpelRecord *recs, size_t n, uint8_t *dst, const u
 typedef struct FFQpelRecord { uint32_t dst_off, src_off; uint8_t kind, sidx, mc, pad; } FFQpelRecord;
 int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *recs, size_t n, uint8_t *dst, const uint8_t *src, ptrdiff_t stride, void *stream);
 
+/* ---- mpegvideo motion compensation (MPEG-1 / MPEG-2, H.263 / MPEG-4 part 2; 8 bit 4:2:0) ------------------------------------------------
+ * ff_mpv_motion() (libavcodec/mpegvideo_motion.c:814-968) for every direction of a macroblock, in ff_mpv_reconstruct_mb's order
+ * (mpegvideo.c:1548-1578): the forward prediction with put (put_no_rnd when no_rounding is set in a P picture), then the backward one
+ * with avg.  One record per inter macroblock, its fields named after the MpegEncContext fields the C function reads.
+ *   MPEG-1 / MPEG-2 (out_format 0): 16X16 in frame pictures; FIELD in frame and field pictures; 16X8 in field pictures; DMV in both.
+ *     A vector whose block leaves [0, h_edge_pos) x [0, v_edge_pos) skips that mpeg_motion call, exactly like the C code (:333-342).
+ *   H.263 / MPEG-4 (out_format 2): 16X16 half- and quarter-sample, 8X8 (4MV) half- and quarter-sample, with the reference's edge
+ *     emulation where it emulates (clamped addressing) and direct reads where it reads directly.
+ * Refused: GMC / sprites, OBMC, H.261, WMV2 mspel, field pictures and field MC in the H.263 family, 4:2:2 / 4:4:4, lowres.  A picture
+ * asking for one of them makes the call return -1 with avb200_last_error() set, and nothing is launched.  A record the kernel cannot
+ * take (an mv_type outside the family's list, mv_dir above 7, a macroblock outside the picture, a direction whose reference planes are
+ * NULL) leaves its macroblock untouched and adds one to *rejected (device uint32).
+ * Memory: the kernel reads each reference plane only inside rows [0, 16 * mb_height] and columns [0, 16 * mb_width] (chroma
+ * [0, 8 * mb_height] x [0, 8 * mb_width]), whatever the records hold: the macroblock-aligned plane plus one row below and one column to
+ * the right.  The C code reads that far directly in one case: in a picture narrower (shorter) than 16 samples, FFMAX(h_edge_pos - 16, 0)
+ * lets a 16x16 H.263 / MPEG-4 vector at 0 read the reference directly, and its 9-sample chroma block ends one column (row) past the
+ * aligned plane.  Elsewhere direct reads may pass h_edge_pos / v_edge_pos but stay inside the aligned plane.  The kernel writes only the
+ * destination macroblocks of accepted records.
+ * Records of one picture run concurrently: a picture holds at most one record per macroblock (two records for the same mb_x, mb_y race,
+ * and the result is undefined).  Pictures of one call run concurrently too, so none may read what another writes: a second field that
+ * predicts from its own first field goes into a later call.  Checked by frame base (dest[0], one line less for a bottom field): two
+ * pictures of a call writing the same frame, a picture whose frame is another's last[0] / next[0] or its own, and a cur[0] other than
+ * that frame are refused. */
+typedef struct FFMpvMCRecord {
+    uint16_t mb_x, mb_y;          /* s->mb_x; the macroblock row in the picture: s->mb_y >> field_pic */
+    uint8_t  mv_dir;              /* s->mv_dir: bit 0 MV_DIR_FORWARD, bit 1 MV_DIR_BACKWARD (bit 2, MV_DIRECT, is ignored) */
+    uint8_t  mv_type;             /* s->mv_type: 0 16X16, 1 8X8, 2 16X8, 3 FIELD, 4 DMV */
+    uint8_t  field_select[2][2];  /* s->field_select */
+    int16_t  mv[2][4][2];         /* s->mv */
+    uint8_t  pad[2];
+} FFMpvMCRecord;
+typedef struct FFMpvMCPicture {
+    uint8_t *dest[3];                   /* s->current_picture.f->data: the bottom field of a field picture starts one line down */
+    const uint8_t *cur[3];              /* s->current_picture_ptr->f->data: the frame's own planes (second field P prediction) */
+    const uint8_t *last[3], *next[3];   /* s->last_picture.f->data, s->next_picture.f->data (NULL where no record uses them) */
+    int linesize, uvlinesize;           /* s->linesize, s->uvlinesize (frame lines) */
+    int pic_linesize, pic_uvlinesize;   /* s->current_picture.f->linesize[0] / [1]: the frame's, doubled in a field picture */
+    int mb_width, mb_height;            /* s->mb_width, s->mb_height (frame macroblocks) */
+    int width, height, h_edge_pos, v_edge_pos;
+    int out_format;                     /* s->out_format: 0 FMT_MPEG1 (MPEG-1 / 2), 2 FMT_H263 (H.263, MPEG-4 part 2); 1 (H.261) is refused */
+    int picture_structure;              /* 1 top field, 2 bottom field, 3 frame */
+    int first_field, b_picture;         /* s->first_field; s->pict_type == AV_PICTURE_TYPE_B */
+    int no_rounding, quarter_sample, workaround_bugs;
+    int chroma_format;                  /* s->chroma_format: 1 (4:2:0) */
+    int obmc, sprite, mspel, lowres;    /* s->obmc; s->pict_type == AV_PICTURE_TYPE_S; s->mspel; avctx->lowres: must be 0 */
+    const FFMpvMCRecord *recs;          /* device; at most one record per macroblock */
+    size_t n_recs;
+} FFMpvMCPicture;
+int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, int n_pictures, uint32_t *rejected, void *stream);
+
+/* The flush point of an mpegvideo decoder back-end: the decoder parses a batch of pictures, records the motion of every inter macroblock
+ * and the coefficient blocks of every coded block, and flushes with one call.  On `stream`, without synchronising: the motion
+ * compensation of every picture (ff_mpv_motion_batch_cuda), then the residual batches in the order given, each through one existing entry
+ * point -- the simple or the Xvid transform, with no inverse quantiser or one of the seven kinds of ff_mpeg_dequant_idct_batch_cuda:
+ *   dequant -1, transform 0: ff_simple_idct_batch_cuda(mode, ...)        dequant k, transform 0: ff_mpeg_dequant_idct_batch_cuda(k, ...)
+ *   dequant -1, transform 1: ff_xvid_idct_batch_cuda(mode, ...)          dequant k, transform 1: ff_mpeg_dequant_xvid_idct_batch_cuda(k, ...)
+ * Intra blocks (idct_put / put_dct) and inter blocks (idct_add / add_dct / add_dequant_dct) go in separate batches, and so do frame and
+ * field DCT blocks: a field-DCT block of a macroblock at dest has dct_linesize = 2 * linesize and its lower blocks start one line down
+ * (mpegvideo.c:1534-1535).  Blocks are addressed through dst_off (byte offsets into `frame`).  Every batch is checked before anything is
+ * launched; a refusal returns -1 and leaves every picture as it was.  A batch its entry point refuses later (its alignment rules) stops
+ * the flush with -1 after the stages before it were enqueued. */
+typedef struct FFMpvResidualBatch {
+    int transform;                       /* 0 simple IDCT, 1 Xvid IDCT */
+    int dequant;                         /* -1: the blocks are dequantised already; 0..6: the inverse quantiser kind fused in front */
+    int mode;                            /* dequant -1: 0 put, 1 add (a fused kind puts for intra kinds, adds for inter kinds) */
+    const FFMpegDequantTables *tables;   /* host struct, dequant >= 0 */
+    const FFMpegDequantBlock *recs;      /* device, dequant >= 0 */
+    int16_t *blocks;                     /* device, n * 64 */
+    uint8_t *frame;                      /* device plane the offsets address */
+    const uint32_t *dst_off;             /* device, n */
+    ptrdiff_t stride;                    /* linesize, or 2 * linesize for field DCT */
+    size_t n;
+    int clear;
+} FFMpvResidualBatch;
+typedef struct FFMpvPictureWork {
+    const FFMpvMCPicture *pictures; int n_pictures;     /* host array: ff_mpv_motion_batch_cuda */
+    uint32_t *rejected;                                 /* device uint32, see ff_mpv_motion_batch_cuda */
+    const FFMpvResidualBatch *residual; int n_residual; /* host array, run in this order after the motion compensation */
+} FFMpvPictureWork;
+int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *work /* host struct */, void *stream);
+
 /* FDCTDSPContext (libavcodec/fdctdsp.h:26-29), in place over n blocks: which 0 = ff_jpeg_fdct_islow_8, 1 =
  * ff_fdct248_islow_8 (jfdctint_template.c:260-398), 2 = ff_fdct_ifast, 3 = ff_fdct_ifast248 (jfdctfst.c:207-332), 4 = ff_jpeg_fdct_islow_10,
  * 5 = ff_fdct248_islow_10 (the BIT_DEPTH 10 instances: PASS1_BITS 1, OUT_SHIFT 2; thread per block, untuned). */

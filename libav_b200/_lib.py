@@ -92,6 +92,8 @@ PROTOTYPES = {
     "ff_me_cmp_enc_batch_cuda": (i32, [i32, i32, vp, vp, vp, pd, i32, vp, sz, vp, vp, vp]),
     "ff_full_search_cuda": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]),
     "ff_hpel_batch_cuda": (i32, [vp, sz, vp, vp, pd, vp]),
+    "ff_mpv_motion_batch_cuda": (i32, [vp, i32, vp, vp]),
+    "ff_mpv_flush_pictures_cuda": (i32, [vp, vp]),
     "ff_fdct_batch_cuda": (i32, [i32, vp, sz, vp]),
     "ff_fft_batch_cuda": (i32, [i32, i32, vp, sz, vp]),
     "ff_mdct_batch_cuda": (i32, [i32, i32, C.c_double, vp, vp, sz, vp]),

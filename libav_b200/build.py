@@ -5,6 +5,7 @@
   oracle/_ref/libavref.so       TEST ONLY: the unmodified reference compiled from /root/reference,
                                 only when that tree is present (never on the GPU box)
   oracle/_ref/libxvidref.so     TEST ONLY: the reference's Xvid IDCT, same conditions
+  oracle/_ref/libmpvmcref.so    TEST ONLY: the reference's mpegvideo motion compensation, same conditions
 All outputs are in-tree so they travel to the GPU box with the snapshot.
 """
 import glob
@@ -85,6 +86,8 @@ def build_oracle_ref(force=False):
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "REF=" + REFERENCE])
     # the Xvid IDCT (oracle/_ref/libxvidref.so), linked against libavref.so
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "xvid.mk", "REF=" + REFERENCE])
+    # the mpegvideo motion compensation (oracle/_ref/libmpvmcref.so), linked against libavref.so
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvmc.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

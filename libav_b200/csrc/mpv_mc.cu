@@ -1,0 +1,155 @@
+// libav_b200/csrc/mpv_mc.cu -- batched mpegvideo motion compensation (ff_mpv_motion, libavcodec/mpegvideo_motion.c) and the picture flush
+// point of an MPEG-1 / MPEG-2 / H.263 / MPEG-4 decoder back-end.
+//
+// One warp per macroblock record, one lane per destination column (mpv_mc_block.cuh).  Up to MPV_PICS_PER_LAUNCH pictures travel as
+// kernel parameters; a warp finds its picture by scanning their record offsets.  The pictures' checks are all made on the host before
+// anything is launched, so a refused call leaves the destination as it was.
+#include "mpv_mc_block.cuh"
+
+namespace avb {
+
+enum { MPV_PICS_PER_LAUNCH = 16 };
+
+struct MpvMcLaunch {
+    MpvMcPic pic[MPV_PICS_PER_LAUNCH];
+    const FFMpvMCRecord *recs[MPV_PICS_PER_LAUNCH];
+    unsigned long long start[MPV_PICS_PER_LAUNCH + 1];     // first warp of each picture; start[n] = warps in the launch
+    int n;
+    uint32_t *rejected;
+};
+
+__global__ void __launch_bounds__(128) mpv_mc_kernel(const __grid_constant__ MpvMcLaunch L)
+{
+    const unsigned long long w = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (w >= L.start[L.n]) return;
+    int p = 0;
+    while (p + 1 < L.n && w >= L.start[p + 1]) p++;
+    const MpvMcPic &P = L.pic[p];
+    const FFMpvMCRecord r = L.recs[p][w - L.start[p]];
+    if (mpv_mc_reject(P, r)) {
+        if ((threadIdx.x & 31) == 0) atomicAdd(L.rejected, 1u);
+        return;
+    }
+    mpv_mc_lane(P, r, threadIdx.x & 31);
+}
+
+namespace {
+
+int refuse(const char *msg) { set_error_msg("ff_mpv_motion_batch_cuda", msg); return -1; }
+
+// the frame the picture writes: dest[0] of a bottom field starts one line into it
+const uint8_t *frame_base(const FFMpvMCPicture &q) { return q.dest[0] - (q.picture_structure == 2 ? q.linesize : 0); }
+
+// the picture-level checks; fills the kernel's view of the picture
+int mpv_picture(const FFMpvMCPicture &q, MpvMcPic &P)
+{
+    if (q.out_format == 1) return refuse("H.261 is not supported");
+    if (q.out_format != 0 && q.out_format != 2) return refuse("out_format must be 0 (MPEG-1 / MPEG-2) or 2 (H.263 / MPEG-4)");
+    if (q.obmc) return refuse("OBMC is not supported");
+    if (q.sprite) return refuse("GMC / sprite pictures are not supported");
+    if (q.mspel) return refuse("WMV2 mspel is not supported");
+    if (q.lowres) return refuse("lowres is not supported");
+    if (q.chroma_format != 1) return refuse("only 4:2:0 chroma is supported");
+    if (q.picture_structure < 1 || q.picture_structure > 3) return refuse("picture_structure must be 1, 2 or 3");
+    const bool frame = q.picture_structure == 3, h263 = q.out_format == 2;
+    if (h263 && !frame) return refuse("field pictures are not supported in the H.263 family");
+    if (q.mb_width <= 0 || q.mb_height <= 0 || q.mb_width > 4096 || q.mb_height > 4096 || (!frame && (q.mb_height & 1)))
+        return refuse("bad macroblock dimensions");
+    if (q.linesize < 16 * q.mb_width + 1 || q.uvlinesize < 8 * q.mb_width + 1 || (q.linesize | q.uvlinesize) < 0)
+        return refuse("linesize / uvlinesize must exceed the macroblock-aligned width");
+    const int k = frame ? 1 : 2;
+    if (q.pic_linesize != k * q.linesize || q.pic_uvlinesize != k * q.uvlinesize)
+        return refuse("pic_linesize must be linesize (frame pictures) or 2 * linesize (field pictures)");
+    if (q.width <= 0 || q.height <= 0 || q.width > 16 * q.mb_width || q.height > 16 * q.mb_height)
+        return refuse("width / height outside the macroblock-aligned picture");
+    const int v_max = frame ? 16 * q.mb_height : 8 * q.mb_height;
+    if (q.h_edge_pos < 2 || q.v_edge_pos < 2 || q.h_edge_pos > 16 * q.mb_width || q.v_edge_pos > v_max)
+        return refuse("h_edge_pos / v_edge_pos outside the macroblock-aligned picture");
+    if (!q.dest[0] || !q.dest[1] || !q.dest[2]) return refuse("NULL destination plane");
+    if (!frame && !q.first_field && (!q.cur[0] || !q.cur[1] || !q.cur[2]))
+        return refuse("a second field needs cur, the planes of its own frame");
+    if (q.n_recs && !q.recs) return refuse("NULL record array");
+    if (q.cur[0] && q.cur[0] != frame_base(q)) return refuse("cur must be the frame that dest belongs to");
+    if (q.last[0] == frame_base(q) || q.next[0] == frame_base(q)) return refuse("last / next is the picture being reconstructed");
+    P = MpvMcPic();
+    for (int i = 0; i < 3; i++) { P.dest[i] = q.dest[i]; P.cur[i] = q.cur[i]; P.ref[0][i] = q.last[i]; P.ref[1][i] = q.next[i]; }
+    P.ls[0] = q.linesize; P.ls[1] = q.uvlinesize; P.pic_k = k;
+    P.mb_w = q.mb_width; P.mb_rows = frame ? q.mb_height : q.mb_height >> 1;
+    P.width = q.width; P.height = q.height; P.h_edge = q.h_edge_pos; P.v_edge = q.v_edge_pos;
+    P.h263 = h263; P.structure = q.picture_structure; P.first_field = q.first_field != 0; P.b_pic = q.b_picture != 0;
+    P.no_rnd = q.no_rounding != 0; P.bugs = q.workaround_bugs; P.qpel = h263 && q.quarter_sample;
+    P.rw[0] = 16 * q.mb_width + 1; P.rh[0] = 16 * q.mb_height + 1;
+    P.rw[1] = 8 * q.mb_width + 1;  P.rh[1] = 8 * q.mb_height + 1;
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace avb
+
+using namespace avb;
+
+extern "C" int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pics, int n, uint32_t *rejected, void *stream)
+{
+    if (n == 0) return 0;
+    if (!pics || n < 0 || !rejected) return refuse("NULL pictures / rejected counter, or a negative count");
+    MpvMcPic *P = new MpvMcPic[n];
+    int rc = 0;
+    for (int i = 0; i < n && !rc; i++) rc = mpv_picture(pics[i], P[i]);
+    // by frame base: two fields of one frame, or a picture whose frame another one predicts from, cannot share a call
+    for (int i = 0; i < n && !rc; i++)
+        for (int j = 0; j < n && !rc; j++) {
+            const uint8_t *b = frame_base(pics[i]);
+            if (i != j && (b == frame_base(pics[j]) || b == pics[j].last[0] || b == pics[j].next[0]))
+                rc = refuse("pictures of one call write the same frame or read each other (a second field predicting from its first field, "
+                            "or a picture predicting from another of the call, goes into a later call)");
+        }
+    if (!rc) {
+        enter();
+        for (int g = 0; g < n && !rc; g += MPV_PICS_PER_LAUNCH) {
+            MpvMcLaunch L;
+            memset(&L, 0, sizeof(L));
+            L.n = n - g < MPV_PICS_PER_LAUNCH ? n - g : MPV_PICS_PER_LAUNCH;
+            L.rejected = rejected;
+            for (int p = 0; p < L.n; p++) {
+                L.pic[p] = P[g + p];
+                L.recs[p] = pics[g + p].recs;
+                L.start[p + 1] = L.start[p] + pics[g + p].n_recs;
+            }
+            const unsigned long long warps = L.start[L.n];
+            if (!warps) continue;
+            AVB_LAUNCH(mpv_mc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
+            rc = check_launch("ff_mpv_motion_batch_cuda");
+        }
+    }
+    delete[] P;
+    return rc;
+}
+
+extern "C" int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *w, void *stream)
+{
+    const char *where = "ff_mpv_flush_pictures_cuda";
+    if (!w || w->n_pictures < 0 || w->n_residual < 0 || (w->n_residual && !w->residual)) { set_error_msg(where, "bad arguments"); return -1; }
+    for (int i = 0; i < w->n_residual; i++) {
+        const FFMpvResidualBatch &b = w->residual[i];
+        if (b.transform < 0 || b.transform > 1 || b.dequant < -1 || b.dequant > 6 || (b.dequant < 0 && b.mode != 0 && b.mode != 1) ||
+            (b.dequant >= 0 && (!b.tables || !b.recs)) || (b.n && (!b.blocks || !b.frame || !b.dst_off))) {
+            set_error_msg(where, "bad residual batch: transform 0 / 1, dequant -1..6, mode 0 / 1, blocks, frame and dst_off set");
+            return -1;
+        }
+    }
+    if (w->n_pictures && ff_mpv_motion_batch_cuda(w->pictures, w->n_pictures, w->rejected, stream)) return -1;
+    for (int i = 0; i < w->n_residual; i++) {
+        const FFMpvResidualBatch &b = w->residual[i];
+        if (!b.n) continue;
+        int rc;
+        if (b.dequant < 0)
+            rc = b.transform ? ff_xvid_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+                             : ff_simple_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
+        else
+            rc = b.transform ? ff_mpeg_dequant_xvid_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+                             : ff_mpeg_dequant_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
+        if (rc) return -1;
+    }
+    return 0;
+}

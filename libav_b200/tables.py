@@ -130,6 +130,30 @@ class FFMpegDequantTables(C.Structure):
                 ("raster_end", C.c_uint8 * 64), ("alternate_scan", C.c_int), ("h263_aic", C.c_int)]
 
 
+class FFMpvMCPicture(C.Structure):
+    """include/avdsp_b200.h FFMpvMCPicture (host struct holding device pointers): ff_mpv_motion_batch_cuda"""
+    _fields_ = [("dest", C.c_void_p * 3), ("cur", C.c_void_p * 3), ("last", C.c_void_p * 3), ("next", C.c_void_p * 3),
+                ("linesize", C.c_int), ("uvlinesize", C.c_int), ("pic_linesize", C.c_int), ("pic_uvlinesize", C.c_int),
+                ("mb_width", C.c_int), ("mb_height", C.c_int), ("width", C.c_int), ("height", C.c_int),
+                ("h_edge_pos", C.c_int), ("v_edge_pos", C.c_int), ("out_format", C.c_int), ("picture_structure", C.c_int),
+                ("first_field", C.c_int), ("b_picture", C.c_int), ("no_rounding", C.c_int), ("quarter_sample", C.c_int),
+                ("workaround_bugs", C.c_int), ("chroma_format", C.c_int), ("obmc", C.c_int), ("sprite", C.c_int), ("mspel", C.c_int),
+                ("lowres", C.c_int), ("recs", C.c_void_p), ("n_recs", C.c_size_t)]
+
+
+class FFMpvResidualBatch(C.Structure):
+    """include/avdsp_b200.h FFMpvResidualBatch: one residual stage of ff_mpv_flush_pictures_cuda"""
+    _fields_ = [("transform", C.c_int), ("dequant", C.c_int), ("mode", C.c_int), ("tables", C.c_void_p), ("recs", C.c_void_p),
+                ("blocks", C.c_void_p), ("frame", C.c_void_p), ("dst_off", C.c_void_p), ("stride", C.c_ssize_t), ("n", C.c_size_t),
+                ("clear", C.c_int)]
+
+
+class FFMpvPictureWork(C.Structure):
+    """include/avdsp_b200.h FFMpvPictureWork (host struct): ff_mpv_flush_pictures_cuda"""
+    _fields_ = [("pictures", C.c_void_p), ("n_pictures", C.c_int), ("rejected", C.c_void_p),
+                ("residual", C.c_void_p), ("n_residual", C.c_int)]
+
+
 class FFMECmpEncState(C.Structure):
     """include/avdsp_b200.h FFMECmpEncState: the MpegEncContext fields quant_psnr / bit / rd read (me_cmp.c:621-782)"""
     _fields_ = [("fdct", C.c_int32), ("dequant", C.c_int32), ("qscale", C.c_int32), ("mb_intra", C.c_int32), ("y_dc_scale", C.c_int32),
