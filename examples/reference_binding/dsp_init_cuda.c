@@ -126,6 +126,23 @@ typedef struct FFMECmpEncView {
     int fdct, dequant, idct_perm_none, plain_quantiser;
 } FFMECmpEncView;
 int ff_me_cmp_enc_init_cuda(MECmpContext *c, struct MpegEncContext *s, const FFMECmpEncView *view);
+/* the quantiser hook: s->dct_quantize / s->fast_dct_quantize (mpegvideo_enc.c:741, :773-779) */
+typedef struct FFMpvQuantView {
+    const int *mb_intra, *y_dc_scale, *c_dc_scale, *h263_aic;
+    const unsigned *lambda2;
+    const int *intra_quant_bias, *inter_quant_bias, *ac_esc_length, *min_qcoeff, *max_qcoeff;
+    int (*const *q_intra_matrix)[64], (*const *q_inter_matrix)[64];
+    const uint16_t *intra_matrix, *inter_matrix;
+    const uint8_t *scantable;
+    uint8_t *const *intra_ac_vlc_length, *const *intra_ac_vlc_last_length, *const *inter_ac_vlc_length, *const *inter_ac_vlc_last_length;
+    int (*const *dct_error_sum)[64];
+    uint16_t (*const *dct_offset)[64];
+    int *dct_count, *coded_score;
+    int (**dct_quantize)(struct MpegEncContext *, int16_t *, int, int, int *);
+    int (**fast_dct_quantize)(struct MpegEncContext *, int16_t *, int, int, int *);
+    int fdct, out_format, mpeg_quant, idct_perm_none, quantizer_noise_shaping, slice_context_count;
+} FFMpvQuantView;
+int ff_mpv_quantize_init_cuda(struct MpegEncContext *s, const FFMpvQuantView *view, int trellis);
 int ff_mpv_encode_init_cuda(MpegEncContext *s)
 {
     FFMECmpEncView v = {
@@ -143,7 +160,25 @@ int ff_mpv_encode_init_cuda(MpegEncContext *s)
         .idct_perm_none = s->idsp.perm_type == FF_IDCT_PERM_NONE,
         .plain_quantiser = s->fast_dct_quantize == ff_dct_quantize_c && !s->dct_error_sum,
     };
-    return ff_me_cmp_enc_init_cuda(&s->mecc, s, &v);      /* -1: the C functions ff_me_cmp_init() installed stay */
+    const int r = ff_me_cmp_enc_init_cuda(&s->mecc, s, &v);      /* -1: the C functions ff_me_cmp_init() installed stay */
+    /* after the metrics, which must still see fast_dct_quantize == ff_dct_quantize_c; the FFMpvQuantView pointers are the same fields */
+    const FFMpvQuantView q = {
+        .mb_intra = &s->mb_intra, .y_dc_scale = &s->y_dc_scale, .c_dc_scale = &s->c_dc_scale, .h263_aic = &s->h263_aic,
+        .lambda2 = &s->lambda2, .intra_quant_bias = &s->intra_quant_bias, .inter_quant_bias = &s->inter_quant_bias,
+        .ac_esc_length = &s->ac_esc_length, .min_qcoeff = &s->min_qcoeff, .max_qcoeff = &s->max_qcoeff,
+        .q_intra_matrix = &s->q_intra_matrix, .q_inter_matrix = &s->q_inter_matrix,
+        .intra_matrix = s->intra_matrix, .inter_matrix = s->inter_matrix, .scantable = s->intra_scantable.scantable,
+        .intra_ac_vlc_length = &s->intra_ac_vlc_length, .intra_ac_vlc_last_length = &s->intra_ac_vlc_last_length,
+        .inter_ac_vlc_length = &s->inter_ac_vlc_length, .inter_ac_vlc_last_length = &s->inter_ac_vlc_last_length,
+        .dct_error_sum = &s->dct_error_sum, .dct_offset = &s->dct_offset, .dct_count = s->dct_count, .coded_score = s->coded_score,
+        .dct_quantize = &s->dct_quantize, .fast_dct_quantize = &s->fast_dct_quantize,
+        .fdct = v.fdct, .out_format = s->out_format, .mpeg_quant = s->mpeg_quant,
+        .idct_perm_none = s->idsp.perm_type == FF_IDCT_PERM_NONE,
+        .quantizer_noise_shaping = s->quantizer_noise_shaping,
+        .slice_context_count = s->slice_context_count,           /* > 1 (slice threads): refused, the C quantisers stay */
+    };
+    ff_mpv_quantize_init_cuda(s, &q, s->avctx->trellis);          /* -1: ff_dct_quantize_c / dct_quantize_trellis_c stay */
+    return r;
 }
 
 /* ---- libswscale (INTEGRATION.md section 4): the whole-frame SwsFunc and the per-line slots ---- */

@@ -430,6 +430,58 @@ void ff_me_cmp_enc_state_free_cuda(void *enc_state);
 int ff_me_cmp_enc_batch_cuda(int kind, int sidx, const void *enc_state, const uint8_t *cur, const uint8_t *ref, ptrdiff_t stride, int h,
                              const FFMECmpRecord *recs, size_t n, int32_t *out, int32_t *last_index, void *stream);
 
+/* ---- the mpegvideo encoders' quantiser (MPEG-1 / MPEG-2, H.263 / MPEG-4 part 2, MJPEG; 8 bit) --------------------------------------------
+ * What encode_mb_internal (libavcodec/mpegvideo_enc.c:2263-2303) does to every coded block between the pixel fetch and the VLC pass:
+ *   s->dct_quantize: the forward DCT (s->fdsp.fdct), denoise_dct_c when noise reduction is on (:3621-3643), then ff_dct_quantize_c
+ *   (:4371-4450) or, with trellis, dct_quantize_trellis_c (:3645-3936); clip_coeffs (:1951-1983) when the quantiser reports overflow;
+ *   dct_single_coeff_elimination (:1895-1949) on inter blocks when the block's threshold (luma for blocks 0-3, chroma for the rest) is not 0.
+ * FFMpvQuantState = the MpegEncContext fields those functions read that stay fixed over a picture, by value: q_intra_matrix / q_inter_matrix
+ * for every qscale as ff_convert_matrix() built them (mpegvideo_enc.c:84-160), scantable = s->intra_scantable.scantable.  The IDCT must not
+ * permute (FF_IDCT_PERM_NONE), so levels come back in raster order exactly as the C code leaves s->block[n].  FFMpvQuantRecord = the fields
+ * that change per macroblock or block.  The trellis also reads the codec's VLC length tables (FFMECmpVlcTables: the same device cache as the
+ * quant_psnr / bit / rd metrics; luma_dc_vlc_length is not read and may be NULL).  Under ff_fdct_ifast the trellis weighs its distortion with
+ * ff_inv_aanscales, which the library derives from its definition (round(4096 / (a(u) a(v))), a(0) = 1, a(k) = sqrt(2) cos(k pi / 16)). */
+typedef struct FFMpvQuantState {
+    int32_t fdct;                                   /* s->fdsp.fdct: 0 ff_jpeg_fdct_islow_8, 2 ff_fdct_ifast */
+    int32_t out_format;                             /* enum OutputFormat (mpegutils.h): 0 FMT_MPEG1, 1 FMT_H261, 2 FMT_H263, 3 FMT_MJPEG */
+    int32_t mpeg_quant, h263_aic;
+    int32_t intra_quant_bias, inter_quant_bias;     /* QUANT_BIAS_SHIFT units; the trellis ignores them (its own thresholds) */
+    int32_t ac_esc_length, min_qcoeff, max_qcoeff;
+    int32_t luma_elim_threshold, chroma_elim_threshold;   /* 0 = off, < 0 = the DC too */
+    int32_t q_intra_matrix[32][64], q_inter_matrix[32][64];
+    uint16_t intra_matrix[64], inter_matrix[64];
+    uint8_t scantable[64];                          /* a permutation of 0..63 with scantable[0] == 0 */
+    uint8_t pad[8];
+} FFMpvQuantState;
+typedef struct FFMpvQuantRecord {                   /* one per block */
+    uint8_t qscale;                                 /* 1..31 */
+    uint8_t intra;                                  /* s->mb_intra */
+    uint8_t dc_scale;                               /* s->y_dc_scale for blocks 0-3, s->c_dc_scale for the others (intra, not h263_aic: >= 1) */
+    uint8_t chroma;                                 /* block index n >= 4: picks the elimination threshold */
+    uint32_t lambda2;                               /* s->lambda2 of the macroblock (trellis) */
+} FFMpvQuantRecord;
+typedef struct FFMpvNoiseReduction {                /* DEVICE pointers: s->dct_offset [2][64], s->dct_error_sum [2][64], s->dct_count [2] */
+    const uint16_t *dct_offset;
+    int32_t *dct_error_sum, *dct_count;
+} FFMpvNoiseReduction;
+/* device-resident copy of a state (one per picture, or per change of matrices); NULL + avb200_last_error() for a bad state: an fdct other
+ * than 0 or 2, an out_format outside 0..3, a scantable that is not a permutation starting at 0.  vlc may be NULL when no call uses trellis. */
+void *ff_mpv_quant_state_cuda(const FFMpvQuantState *state, const FFMECmpVlcTables *vlc);
+void ff_mpv_quant_state_free_cuda(void *quant_state);
+/* n blocks, one thread each, on `stream` without synchronising.  Input: s1 == NULL -> blocks[i] already holds what get_pixels /
+ * diff_pixels left there; otherwise the kernel fetches block i itself from s1 + off1[i] (minus s2 + off2[i] when s2 != NULL; off2 NULL = the
+ * same offsets), as ff_pixblock_fdct_batch_cuda does.  trellis 0 = ff_dct_quantize_c, 1 = dct_quantize_trellis_c.  Output: blocks[i] =
+ * the levels after the clip and the elimination (raster order), last_index[i] = s->block_last_index[n] after them, coded_score[i] (optional)
+ * = s->coded_score[n] where the trellis writes it (it is left as it was where the C code leaves it).  nr (host struct of device pointers,
+ * NULL = off): the dct_offset the blocks are denoised with, and dct_error_sum / dct_count, which are added to (int32 adds: the C result
+ * whatever the block order).  A record with qscale outside 1..31 or an intra dc_scale of 0 (without h263_aic) leaves its block, last_index,
+ * coded_score and the sums alone: the records are device memory, so unlike the checks below this one is made by the kernel, per block,
+ * and the call still returns 0.  Returns 0 (n == 0 too), or -1 with avb200_last_error() set and nothing launched: no state, trellis on a
+ * state without VLC tables, blocks not 16-byte aligned, a NULL buffer. */
+int ff_mpv_dct_quantize_batch_cuda(const void *quant_state, int trellis, const FFMpvQuantRecord *recs, const uint8_t *s1, const uint8_t *s2,
+                                   const uint32_t *off1, const uint32_t *off2, ptrdiff_t stride, int16_t *blocks, size_t n,
+                                   int32_t *last_index, int32_t *coded_score, const FFMpvNoiseReduction *nr, void *stream);
+
 /* Exhaustive search (libavcodec/motion_est_template.c:620-655) for every 16x16 macroblock of rows [mb_y0, mb_y1):
  * candidates within +-range (16) clipped so the block stays inside the picture (get_limits, motion_est.c:517-548),
  * score = pix_abs[0][0] (h = 16), penalty_factor 0, strict-< minimum in raster order (mathops.h:133-140).
@@ -644,6 +696,38 @@ typedef struct FFMECmpEncView {
 } FFMECmpEncView;
 int ff_me_cmp_enc_init_cuda(MECmpContext *c, struct MpegEncContext *s, const FFMECmpEncView *view);
 void ff_me_cmp_enc_uninit_cuda(struct MpegEncContext *s);
+/* The arch hook of the encoder's quantiser (same place as ff_mpv_encode_init_x86, libavcodec/mpegvideo_enc.c:741, :773-779): fills
+ * *view->fast_dct_quantize with the plain slot and *view->dct_quantize with the trellis slot when `trellis` (avctx->trellis) is set, the
+ * plain one otherwise.  The slots have the reference's signature and apply noise reduction themselves when *view->dct_error_sum is set, as the
+ * C quantisers do.  Like the metric slots they read the live context through `view` on every call (one block: stage, copy, kernel, copy
+ * back, synchronise).  Returns 0, or -1 with the context untouched for: a permuting IDCT, an fdct other than islow / ifast (FF_DCT_FAAN,
+ * a 10-bit encoder), quantizer_noise_shaping, slice threading (slice_context_count > 1), a NULL view pointer.  Slice threading is refused
+ * because the view points into the one context it was made from: ff_update_duplicate_context copies the slots into the per-thread
+ * contexts, whose mb_intra, lambda2, coded_score and noise-reduction sums are their own.  Such an encoder keeps the C quantisers (the
+ * batched call serves it instead).  Call it after ff_me_cmp_enc_init_cuda, which must still see
+ * fast_dct_quantize == ff_dct_quantize_c. */
+typedef struct FFMpvQuantView {
+    const int *mb_intra, *y_dc_scale, *c_dc_scale, *h263_aic;
+    const unsigned *lambda2;
+    const int *intra_quant_bias, *inter_quant_bias, *ac_esc_length, *min_qcoeff, *max_qcoeff;
+    int (*const *q_intra_matrix)[64], (*const *q_inter_matrix)[64];     /* &s->q_intra_matrix, &s->q_inter_matrix */
+    const uint16_t *intra_matrix, *inter_matrix;
+    const uint8_t *scantable;                                            /* s->intra_scantable.scantable */
+    uint8_t *const *intra_ac_vlc_length, *const *intra_ac_vlc_last_length, *const *inter_ac_vlc_length, *const *inter_ac_vlc_last_length;
+    int (*const *dct_error_sum)[64];                                     /* &s->dct_error_sum (NULL inside = noise reduction off) */
+    uint16_t (*const *dct_offset)[64];                                   /* &s->dct_offset */
+    int *dct_count;                                                      /* s->dct_count */
+    int *coded_score;                                                    /* s->coded_score */
+    int (**dct_quantize)(struct MpegEncContext *, int16_t *, int, int, int *);       /* &s->dct_quantize */
+    int (**fast_dct_quantize)(struct MpegEncContext *, int16_t *, int, int, int *);  /* &s->fast_dct_quantize */
+    int fdct;                                                            /* 0 ff_jpeg_fdct_islow_8, 2 ff_fdct_ifast, anything else refused */
+    int out_format, mpeg_quant;                                          /* s->out_format, s->mpeg_quant */
+    int idct_perm_none;                                                  /* s->idsp.perm_type == FF_IDCT_PERM_NONE */
+    int quantizer_noise_shaping;                                         /* s->quantizer_noise_shaping */
+    int slice_context_count;                                             /* s->slice_context_count: must be 1 (see above) */
+} FFMpvQuantView;
+int ff_mpv_quantize_init_cuda(struct MpegEncContext *s, const FFMpvQuantView *view, int trellis);
+void ff_mpv_quantize_uninit_cuda(struct MpegEncContext *s);
 /* libavcodec/h264dsp.c:57-143, h264qpel.c:36-89, h264chroma.c:32-55, hpeldsp.c:338-366.  bit_depth 8, and 9 / 10 (the reference's BIT_DEPTH > 8
  * instances: uint8_t * arguments point at uint16 samples, int16_t * at int32 coefficients, strides stay in bytes).  ff_h264dsp_init_cuda fills
  * every entry ff_h264dsp_init fills (mbaff loop filters and startcode_find_candidate included); chroma_format_idc > 1 selects the

@@ -90,6 +90,9 @@ PROTOTYPES = {
     "ff_me_cmp_enc_state_cuda": (vp, [vp, vp]),
     "ff_me_cmp_enc_state_free_cuda": (None, [vp]),
     "ff_me_cmp_enc_batch_cuda": (i32, [i32, i32, vp, vp, vp, pd, i32, vp, sz, vp, vp, vp]),
+    "ff_mpv_quant_state_cuda": (vp, [vp, vp]),
+    "ff_mpv_quant_state_free_cuda": (None, [vp]),
+    "ff_mpv_dct_quantize_batch_cuda": (i32, [vp, i32, vp, vp, vp, vp, vp, pd, vp, sz, vp, vp, vp, vp]),
     "ff_full_search_cuda": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]),
     "ff_hpel_batch_cuda": (i32, [vp, sz, vp, vp, pd, vp]),
     "ff_mpv_motion_batch_cuda": (i32, [vp, i32, vp, vp]),
@@ -115,6 +118,8 @@ PROTOTYPES = {
     "ff_me_cmp_init_cuda": (None, [vp]),
     "ff_me_cmp_enc_init_cuda": (i32, [vp, vp, vp]),
     "ff_me_cmp_enc_uninit_cuda": (None, [vp]),
+    "ff_mpv_quantize_init_cuda": (i32, [vp, vp, i32]),
+    "ff_mpv_quantize_uninit_cuda": (None, [vp]),
     "ff_h264dsp_init_cuda": (None, [vp, i32, i32]),
     "ff_h264qpel_init_cuda": (None, [vp, i32]),
     "ff_h264chroma_init_cuda": (None, [vp, i32]),

@@ -6,6 +6,7 @@
                                 only when that tree is present (never on the GPU box)
   oracle/_ref/libxvidref.so     TEST ONLY: the reference's Xvid IDCT, same conditions
   oracle/_ref/libmpvmcref.so    TEST ONLY: the reference's mpegvideo motion compensation, same conditions
+  oracle/_ref/libmpvqref.so     TEST ONLY: the reference's encoder quantisers (plain, trellis, noise reduction), same conditions
 All outputs are in-tree so they travel to the GPU box with the snapshot.
 """
 import glob
@@ -88,6 +89,8 @@ def build_oracle_ref(force=False):
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "xvid.mk", "REF=" + REFERENCE])
     # the mpegvideo motion compensation (oracle/_ref/libmpvmcref.so), linked against libavref.so
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvmc.mk", "REF=" + REFERENCE])
+    # the encoder quantisers (oracle/_ref/libmpvqref.so), linked against libavref.so
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvq.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

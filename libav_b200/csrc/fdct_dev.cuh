@@ -61,4 +61,77 @@ __device__ __forceinline__ void ifast_1d(const int (&in)[8], int (&out)[8])
     out[5] = z13 + z2; out[3] = z13 - z2; out[1] = z11 + z4; out[7] = z11 - z4;
 }
 
+// The two passes of the 2-D forward DCT as FDCTDSPContext.fdct runs them on an int16 block (FDCT as in ff_fdct_batch_cuda 0..3):
+// fdct_row = the row pass of one row with the int16 write-back the C code does between the passes, fdct_cols = the column pass over a
+// block held in registers (not yet truncated: the caller's int16 store does that).
+template <int FDCT>
+__device__ __forceinline__ void fdct_row(const int (&in)[8], int (&out)[8])
+{
+    int o[8];
+    if (FDCT < 2) islow_1d<4, 9>(in, o); else ifast_1d(in, o);
+#pragma unroll
+    for (int k = 0; k < 8; k++) out[k] = (int)(int16_t)o[k];
+}
+template <int FDCT>
+__device__ __forceinline__ void fdct_cols(int (&m)[8][8])
+{
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+        int in[8], o[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) in[k] = m[k][c];
+        if (FDCT == 0) islow_1d<-4, 17>(in, o);
+        else if (FDCT == 1) col_248<false>(in, o);
+        else if (FDCT == 2) ifast_1d(in, o);
+        else col_248<true>(in, o);
+#pragma unroll
+        for (int k = 0; k < 8; k++) m[k][c] = o[k];
+    }
+}
+
+// PixblockDSPContext.get_pixels / diff_pixels (pixblockdsp_template.c:24-66) of the 8x8 block at a (minus the one at b, b != NULL),
+// optionally followed by the forward DCT in the same thread (FDCT as in ff_fdct_batch_cuda 0..3; < 0: the samples / differences): the
+// spatial block never exists as int16 in memory.  m holds what the C code leaves in its int16 block (the column pass is not yet truncated).
+// Shared by pixblock_kernel (me_cmp.cu) and the quantiser's front end (mpv_quant.cu).
+template <int FDCT>
+__device__ __forceinline__ void pixblock_fetch(const uint8_t *a, const uint8_t *b, ptrdiff_t stride, int (&m)[8][8])
+{
+    const bool vec = !(((uintptr_t)a | (uintptr_t)b | (uintptr_t)stride) & 7);
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        int in[8];
+        if (vec) {
+            const uint2 pa = *reinterpret_cast<const uint2 *>(a + r * stride);
+#pragma unroll
+            for (int k = 0; k < 4; k++) { in[k] = byte_of(pa.x, k); in[4 + k] = byte_of(pa.y, k); }
+            if (b) {
+                const uint2 pb = *reinterpret_cast<const uint2 *>(b + r * stride);
+#pragma unroll
+                for (int k = 0; k < 4; k++) { in[k] -= byte_of(pb.x, k); in[4 + k] -= byte_of(pb.y, k); }
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; k++) in[k] = a[r * stride + k] - (b ? b[r * stride + k] : 0);
+        }
+        if (FDCT < 0) {
+#pragma unroll
+            for (int k = 0; k < 8; k++) m[r][k] = in[k];
+        } else fdct_row<FDCT>(in, m[r]);
+    }
+    if (FDCT >= 0) fdct_cols<FDCT>(m);
+}
+
+// the forward DCT of an int16 block in memory (16-byte aligned), into registers as pixblock_fetch leaves them
+template <int FDCT>
+__device__ __forceinline__ void fdct_load(const int16_t *b, int (&m)[8][8])
+{
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const uint4 v = reinterpret_cast<const uint4 *>(b)[r];
+        const int in[8] = { lo16s(v.x), hi16s(v.x), lo16s(v.y), hi16s(v.y), lo16s(v.z), hi16s(v.z), lo16s(v.w), hi16s(v.w) };
+        fdct_row<FDCT>(in, m[r]);
+    }
+    fdct_cols<FDCT>(m);
+}
+
 }  // namespace avb

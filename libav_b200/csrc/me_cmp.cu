@@ -242,26 +242,7 @@ __global__ void __launch_bounds__(128) fdct_kernel(int16_t *__restrict__ blocks,
     if (i >= n) return;
     int16_t *b = blocks + 64 * i;
     int m[8][8];
-#pragma unroll
-    for (int r = 0; r < 8; r++) {
-        const uint4 v = reinterpret_cast<const uint4 *>(b)[r];
-        int in[8] = { lo16s(v.x), hi16s(v.x), lo16s(v.y), hi16s(v.y), lo16s(v.z), hi16s(v.z), lo16s(v.w), hi16s(v.w) }, o[8];
-        if (WHICH < 2) islow_1d<4, 9>(in, o); else ifast_1d(in, o);
-#pragma unroll
-        for (int k = 0; k < 8; k++) m[r][k] = (int)(int16_t)o[k];
-    }
-#pragma unroll
-    for (int c = 0; c < 8; c++) {
-        int in[8], o[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) in[k] = m[k][c];
-        if (WHICH == 0) islow_1d<-4, 17>(in, o);
-        else if (WHICH == 1) col_248<false>(in, o);
-        else if (WHICH == 2) ifast_1d(in, o);
-        else col_248<true>(in, o);
-#pragma unroll
-        for (int k = 0; k < 8; k++) m[k][c] = o[k];
-    }
+    fdct_load<WHICH>(b, m);
 #pragma unroll
     for (int r = 0; r < 8; r++)
         reinterpret_cast<uint4 *>(b)[r] = make_uint4(pack16(m[r][0], m[r][1]), pack16(m[r][2], m[r][3]), pack16(m[r][4], m[r][5]), pack16(m[r][6], m[r][7]));
@@ -277,48 +258,8 @@ pixblock_kernel(const uint8_t *__restrict__ s1, const uint8_t *__restrict__ s2, 
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint8_t *a = s1 + off1[i], *b = s2 ? s2 + (off2 ? off2[i] : off1[i]) : nullptr;
-    const bool vec = !(((uintptr_t)a | (uintptr_t)b | (uintptr_t)stride) & 7);
     int m[8][8];
-#pragma unroll
-    for (int r = 0; r < 8; r++) {
-        int in[8];
-        if (vec) {
-            const uint2 pa = *reinterpret_cast<const uint2 *>(a + r * stride);
-#pragma unroll
-            for (int k = 0; k < 4; k++) { in[k] = byte_of(pa.x, k); in[4 + k] = byte_of(pa.y, k); }
-            if (b) {
-                const uint2 pb = *reinterpret_cast<const uint2 *>(b + r * stride);
-#pragma unroll
-                for (int k = 0; k < 4; k++) { in[k] -= byte_of(pb.x, k); in[4 + k] -= byte_of(pb.y, k); }
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < 8; k++) in[k] = a[r * stride + k] - (b ? b[r * stride + k] : 0);
-        }
-        if (FDCT < 0) {
-#pragma unroll
-            for (int k = 0; k < 8; k++) m[r][k] = in[k];
-        } else {
-            int o[8];
-            if (FDCT < 2) islow_1d<4, 9>(in, o); else ifast_1d(in, o);
-#pragma unroll
-            for (int k = 0; k < 8; k++) m[r][k] = (int)(int16_t)o[k];
-        }
-    }
-    if (FDCT >= 0) {
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-            int in[8], o[8];
-#pragma unroll
-            for (int k = 0; k < 8; k++) in[k] = m[k][c];
-            if (FDCT == 0) islow_1d<-4, 17>(in, o);
-            else if (FDCT == 1) col_248<false>(in, o);
-            else if (FDCT == 2) ifast_1d(in, o);
-            else col_248<true>(in, o);
-#pragma unroll
-            for (int k = 0; k < 8; k++) m[k][c] = o[k];
-        }
-    }
+    pixblock_fetch<FDCT>(a, b, stride, m);
     int16_t *d = blocks + 64 * i;
 #pragma unroll
     for (int r = 0; r < 8; r++)

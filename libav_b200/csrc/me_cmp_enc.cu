@@ -17,6 +17,7 @@
 // metrics: thousands of records per launch, instruction-bound (two transforms + two scans per block); the state lives in device memory.
 #include "common.cuh"
 #include "fdct_dev.cuh"
+#include "mpv_quant.cuh"
 #include "scratch.h"
 #include "../../include/avdsp_b200.h"
 #include <map>
@@ -30,9 +31,48 @@ struct EncDev {
     const uint8_t *vlc[5];          // device copies: intra len, intra last, inter len, inter last, luma dc
 };
 
+// ---- device copies of the codec's VLC length tables, keyed by their host addresses (static tables in the reference) ----
+// The per-call slots look the copy up by address alone; the two places a caller announces tables (ff_me_cmp_enc_init_cuda, ff_me_cmp_enc_state_cuda)
+// also compare a checksum of the host bytes with the one taken at upload, so memory that was freed and reused for other tables gets a fresh copy
+// (the old one stays alive for the states that point at it).
+// (shared with mpv_quant.cu, declared in mpv_quant.cuh)
+struct VlcKey { const uint8_t *p[5]; bool operator<(const VlcKey &o) const { return memcmp(p, o.p, sizeof(p)) < 0; } };
+struct VlcCopy { uint8_t *d; uint64_t sum; };
 namespace {
+std::mutex g_vlc_mu;
+std::map<VlcKey, VlcCopy> g_vlc;
+constexpr size_t VLC_BYTES = 4 * 64 * 128 + 512;
 
-constexpr int QSHIFT = 22, BIAS_SHIFT = 8;     // QMAT_SHIFT, QUANT_BIAS_SHIFT (mpegvideo_enc.c:65-68)
+uint64_t vlc_checksum(const VlcKey &key)
+{
+    uint64_t h = 0xcbf29ce484222325ull;
+    for (int k = 0; k < 5; k++) {
+        const size_t n = k < 4 ? 8192 : 512;
+        for (size_t i = 0; i < n; i += 8) { uint64_t w; memcpy(&w, key.p[k] + i, 8); h = (h ^ w) * 0x100000001b3ull; h ^= h >> 29; }
+    }
+    return h;
+}
+}  // namespace
+
+const uint8_t *vlc_device(const FFMECmpVlcTables *v, const char *where, bool verify)
+{
+    const VlcKey key = { { v->intra_ac_vlc_length, v->intra_ac_vlc_last_length, v->inter_ac_vlc_length, v->inter_ac_vlc_last_length, v->luma_dc_vlc_length } };
+    for (int k = 0; k < 5; k++) if (!key.p[k]) { set_error_msg(where, "a VLC length table is NULL"); return nullptr; }
+    std::lock_guard<std::mutex> lk(g_vlc_mu);
+    auto it = g_vlc.find(key);
+    if (it != g_vlc.end() && !verify) return it->second.d;
+    const uint64_t sum = vlc_checksum(key);
+    if (it != g_vlc.end() && it->second.sum == sum) return it->second.d;
+    uint8_t *d = nullptr;
+    if (cudaMalloc(&d, VLC_BYTES) != cudaSuccess) { set_error(where, cudaGetLastError()); return nullptr; }
+    bool ok = true;
+    for (int k = 0; k < 4; k++) ok = ok && cudaMemcpy(d + (size_t)k * 8192, key.p[k], 8192, cudaMemcpyHostToDevice) == cudaSuccess;
+    ok = ok && cudaMemcpy(d + 4 * 8192, key.p[4], 512, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (!ok) { set_error(where, cudaGetLastError()); cudaFree(d); return nullptr; }
+    g_vlc[key] = VlcCopy{ d, sum };
+    return d;
+}
+namespace {
 
 // ff_simple_idct_8 on a thread (libavcodec/simple_idct_template.c, BIT_DEPTH 8: W4 = 16383, ROW_SHIFT 11, COL_SHIFT 20, DC_SHIFT 3)
 __device__ inline void enc_idct_rows(int16_t *b)
@@ -111,23 +151,9 @@ __device__ inline int enc_block(const EncDev &E, int kind, const uint8_t *s1, co
     const bool intra = kind != 14 && S.mb_intra != 0;            // quant_psnr clears s->mb_intra first (:629)
     // ---- ff_dct_quantize_c ----
     enc_fdct(t, S.fdct == 2);
-    const int32_t *qmat = intra ? S.q_intra_matrix : S.q_inter_matrix;
-    const int bias = (intra ? S.intra_quant_bias : S.inter_quant_bias) * (1 << (QSHIFT - BIAS_SHIFT));
-    const unsigned t1 = (1u << QSHIFT) - (unsigned)bias - 1u, t2 = t1 << 1;
-    last = intra ? 0 : -1;
-    if (intra) {
-        const int q = (S.h263_aic ? 1 : S.y_dc_scale) << 3;      // n = 0: a luma block (:4389-4396)
-        t[0] = (int16_t)((t[0] + (q >> 1)) / q);
-    }
-    for (int i = intra ? 1 : 0; i < 64; i++) {
-        const int j = S.scantable[i];
-        const int level = (int)((unsigned)(int)t[j] * (unsigned)qmat[j]);
-        if ((unsigned)level + t1 > t2) {
-            const int m = level > 0 ? (int)((unsigned)bias + (unsigned)level) >> QSHIFT : (int)((unsigned)bias - (unsigned)level) >> QSHIFT;
-            t[j] = (int16_t)(level > 0 ? m : -m);
-            last = i;
-        } else t[j] = 0;
-    }
+    int kept_or;                                                  // (unused: these metrics never clip; n = 0, a luma block, :4389-4396)
+    last = mpv_quantize(t, intra, (S.h263_aic ? 1 : S.y_dc_scale) << 3, intra ? S.q_intra_matrix : S.q_inter_matrix,
+                        intra ? S.intra_quant_bias : S.inter_quant_bias, S.scantable, kept_or);
     // ---- VLC bits (bit8x8_c / rd8x8_c) ----
     int bits = 0;
     if (kind != 14) {
@@ -209,44 +235,6 @@ bool state_ok(const FFMECmpEncState *s, const char *where)
     return true;
 }
 
-// ---- device copies of the codec's VLC length tables, keyed by their host addresses (static tables in the reference) ----
-// The per-call slots look the copy up by address alone; the two places a caller announces tables (ff_me_cmp_enc_init_cuda, ff_me_cmp_enc_state_cuda)
-// also compare a checksum of the host bytes with the one taken at upload, so memory that was freed and reused for other tables gets a fresh copy
-// (the old one stays alive for the states that point at it).
-struct VlcKey { const uint8_t *p[5]; bool operator<(const VlcKey &o) const { return memcmp(p, o.p, sizeof(p)) < 0; } };
-struct VlcCopy { uint8_t *d; uint64_t sum; };
-std::mutex g_vlc_mu;
-std::map<VlcKey, VlcCopy> g_vlc;
-constexpr size_t VLC_BYTES = 4 * 64 * 128 + 512;
-
-uint64_t vlc_checksum(const VlcKey &key)
-{
-    uint64_t h = 0xcbf29ce484222325ull;
-    for (int k = 0; k < 5; k++) {
-        const size_t n = k < 4 ? 8192 : 512;
-        for (size_t i = 0; i < n; i += 8) { uint64_t w; memcpy(&w, key.p[k] + i, 8); h = (h ^ w) * 0x100000001b3ull; h ^= h >> 29; }
-    }
-    return h;
-}
-
-const uint8_t *vlc_device(const FFMECmpVlcTables *v, const char *where, bool verify = false)
-{
-    const VlcKey key = { { v->intra_ac_vlc_length, v->intra_ac_vlc_last_length, v->inter_ac_vlc_length, v->inter_ac_vlc_last_length, v->luma_dc_vlc_length } };
-    for (int k = 0; k < 5; k++) if (!key.p[k]) { set_error_msg(where, "a VLC length table is NULL"); return nullptr; }
-    std::lock_guard<std::mutex> lk(g_vlc_mu);
-    auto it = g_vlc.find(key);
-    if (it != g_vlc.end() && !verify) return it->second.d;
-    const uint64_t sum = vlc_checksum(key);
-    if (it != g_vlc.end() && it->second.sum == sum) return it->second.d;
-    uint8_t *d = nullptr;
-    if (cudaMalloc(&d, VLC_BYTES) != cudaSuccess) { set_error(where, cudaGetLastError()); return nullptr; }
-    bool ok = true;
-    for (int k = 0; k < 4; k++) ok = ok && cudaMemcpy(d + (size_t)k * 8192, key.p[k], 8192, cudaMemcpyHostToDevice) == cudaSuccess;
-    ok = ok && cudaMemcpy(d + 4 * 8192, key.p[4], 512, cudaMemcpyHostToDevice) == cudaSuccess;
-    if (!ok) { set_error(where, cudaGetLastError()); cudaFree(d); return nullptr; }
-    g_vlc[key] = VlcCopy{ d, sum };
-    return d;
-}
 void fill_vlc(EncDev &e, const uint8_t *d) { for (int k = 0; k < 5; k++) e.vlc[k] = d ? d + (size_t)k * 8192 : nullptr; }
 
 // ---- slots ----

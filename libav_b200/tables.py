@@ -176,6 +176,38 @@ class FFMECmpEncView(C.Structure):
         [(n, C.c_int) for n in ("fdct", "dequant", "idct_perm_none", "plain_quantiser")]
 
 
+class FFMpvQuantState(C.Structure):
+    """include/avdsp_b200.h FFMpvQuantState: the MpegEncContext fields the encoder's quantisers read that stay fixed over a picture"""
+    _fields_ = [(n, C.c_int32) for n in ("fdct", "out_format", "mpeg_quant", "h263_aic", "intra_quant_bias", "inter_quant_bias", "ac_esc_length",
+                                         "min_qcoeff", "max_qcoeff", "luma_elim_threshold", "chroma_elim_threshold")] + \
+        [("q_intra_matrix", (C.c_int32 * 64) * 32), ("q_inter_matrix", (C.c_int32 * 64) * 32), ("intra_matrix", C.c_uint16 * 64),
+         ("inter_matrix", C.c_uint16 * 64), ("scantable", C.c_uint8 * 64), ("pad", C.c_uint8 * 8)]
+
+
+class FFMpvQuantRecord(C.Structure):
+    """include/avdsp_b200.h FFMpvQuantRecord (8 bytes, one per block)"""
+    _fields_ = [("qscale", C.c_uint8), ("intra", C.c_uint8), ("dc_scale", C.c_uint8), ("chroma", C.c_uint8), ("lambda2", C.c_uint32)]
+
+
+class FFMpvNoiseReduction(C.Structure):
+    """include/avdsp_b200.h FFMpvNoiseReduction: device pointers to dct_offset [2][64], dct_error_sum [2][64], dct_count [2]"""
+    _fields_ = [("dct_offset", C.c_void_p), ("dct_error_sum", C.c_void_p), ("dct_count", C.c_void_p)]
+
+
+class FFMpvQuantView(C.Structure):
+    """include/avdsp_b200.h FFMpvQuantView: host pointers into a live MpegEncContext"""
+    _fields_ = [(n, C.c_void_p) for n in ("mb_intra", "y_dc_scale", "c_dc_scale", "h263_aic", "lambda2", "intra_quant_bias", "inter_quant_bias",
+                                          "ac_esc_length", "min_qcoeff", "max_qcoeff", "q_intra_matrix", "q_inter_matrix", "intra_matrix",
+                                          "inter_matrix", "scantable", "intra_ac_vlc_length", "intra_ac_vlc_last_length", "inter_ac_vlc_length",
+                                          "inter_ac_vlc_last_length", "dct_error_sum", "dct_offset", "dct_count", "coded_score",
+                                          "dct_quantize", "fast_dct_quantize")] + \
+        [(n, C.c_int) for n in ("fdct", "out_format", "mpeg_quant", "idct_perm_none", "quantizer_noise_shaping", "slice_context_count")]
+
+
+# the reference's s->dct_quantize signature (mpegvideo.h:499)
+DCT_QUANTIZE_FUNC = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int))
+
+
 _p4 = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t)
 _p8l = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_ssize_t)
 _p8 = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t)
