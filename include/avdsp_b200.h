@@ -509,7 +509,12 @@ int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *recs, size_t n, uint8_t *dst, c
  *     A vector whose block leaves [0, h_edge_pos) x [0, v_edge_pos) skips that mpeg_motion call, exactly like the C code (:333-342).
  *   H.263 / MPEG-4 (out_format 2): 16X16 half- and quarter-sample, 8X8 (4MV) half- and quarter-sample, with the reference's edge
  *     emulation where it emulates (clamped addressing) and direct reads where it reads directly.
- * Refused: GMC / sprites, OBMC, H.261, WMV2 mspel, field pictures and field MC in the H.263 family, 4:2:2 / 4:4:4, lowres.  A picture
+ * OBMC: a P picture with obmc set (out_format 2, half-sample, obmc_recs given) runs apply_obmc for each record instead, from its
+ *   FFMpvOBMCRecord: the four 8x8 luma blocks as put_obmc weighted sums of hpel_motion predictions (put_no_rnd under no_rounding), chroma
+ *   through chroma_4mv_motion with the sum of the four own vectors -- also for a 16X16 macroblock.  Its records must be forward-only
+ *   (mv_dir & 3 == 1); others count as rejected.  obmc is ignored in B pictures, as in the C code.
+ * Refused: GMC / sprites, OBMC in a quarter-sample, MPEG-1 / 2 or obmc_recs-less P picture, H.261, WMV2 mspel, field pictures and field
+ * MC in the H.263 family, 4:2:2 / 4:4:4, lowres.  A picture
  * asking for one of them makes the call return -1 with avb200_last_error() set, and nothing is launched.  A record the kernel cannot
  * take (an mv_type outside the family's list, mv_dir above 7, a macroblock outside the picture, a direction whose reference planes are
  * NULL) leaves its macroblock untouched and adds one to *rejected (device uint32).
@@ -532,6 +537,19 @@ typedef struct FFMpvMCRecord {
     int16_t  mv[2][4][2];         /* s->mv */
     uint8_t  pad[2];
 } FFMpvMCRecord;
+/* H.263 overlapped block motion compensation (Annex F; Intel H.263; RV10 micro-version 2): apply_obmc (mpegvideo_motion.c:643-728), which
+ * replaces ff_mpv_motion's prediction in a P picture with obmc set.  It reads current_picture.motion_val[0] and mb_type at the moment the
+ * decoder reconstructs the macroblock, and the right neighbour's entries there are not always final (preview_obmc, ituh263dec.c:339-400,
+ * is skipped after a skipped macroblock and for the last macroblock of a GOB), so the record carries raw copies of what it reads; the
+ * kernel makes the substitutions of :674-700 (a neighbour outside the picture or IS_INTRA is replaced by the macroblock's own vectors).
+ * With b8_stride = s->b8_stride, mot_xy = 2 * mb_x + 2 * mb_y * b8_stride and xy = mb_x + mb_y * mb_stride: */
+typedef struct FFMpvOBMCRecord {
+    int16_t mv[4][2];             /* motion_val[0][mot_xy], [mot_xy + 1], [mot_xy + b8_stride], [mot_xy + b8_stride + 1] */
+    int16_t top[2][2];            /* motion_val[0][mot_xy - b8_stride], [mot_xy - b8_stride + 1] (read when mb_y > 0) */
+    int16_t left[2][2];           /* motion_val[0][mot_xy - 1], [mot_xy - 1 + b8_stride] (read when mb_x > 0) */
+    int16_t right[2][2];          /* motion_val[0][mot_xy + 2], [mot_xy + 2 + b8_stride] (read when mb_x + 1 < mb_width) */
+    uint32_t mb_type_top, mb_type_left, mb_type_right;  /* mb_type[xy - mb_stride], [xy - 1], [xy + 1] */
+} FFMpvOBMCRecord;
 typedef struct FFMpvMCPicture {
     uint8_t *dest[3];                   /* s->current_picture.f->data: the bottom field of a field picture starts one line down */
     const uint8_t *cur[3];              /* s->current_picture_ptr->f->data: the frame's own planes (second field P prediction) */
@@ -548,6 +566,7 @@ typedef struct FFMpvMCPicture {
     int obmc, sprite, mspel, lowres;    /* s->obmc; s->pict_type == AV_PICTURE_TYPE_S; s->mspel; avctx->lowres: must be 0 */
     const FFMpvMCRecord *recs;          /* device; at most one record per macroblock */
     size_t n_recs;
+    const FFMpvOBMCRecord *obmc_recs;   /* device, one per record in the same order, read when obmc is set in a P picture; else NULL */
 } FFMpvMCPicture;
 int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, int n_pictures, uint32_t *rejected, void *stream);
 
@@ -561,7 +580,8 @@ int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, in
  * field DCT blocks: a field-DCT block of a macroblock at dest has dct_linesize = 2 * linesize and its lower blocks start one line down
  * (mpegvideo.c:1534-1535).  Blocks are addressed through dst_off (byte offsets into `frame`).  Every batch is checked before anything is
  * launched; a refusal returns -1 and leaves every picture as it was.  A batch its entry point refuses later (its alignment rules) stops
- * the flush with -1 after the stages before it were enqueued. */
+ * the flush with -1 after the stages before it were enqueued.  Then, when loop_filter is set, the H.263 deblocking filter of those pictures
+ * (ff_h263_loop_filter_batch_cuda), checked with everything else before the first stage is enqueued. */
 typedef struct FFMpvResidualBatch {
     int transform;                       /* 0 simple IDCT, 1 Xvid IDCT */
     int dequant;                         /* -1: the blocks are dequantised already; 0..6: the inverse quantiser kind fused in front */
@@ -575,10 +595,32 @@ typedef struct FFMpvResidualBatch {
     size_t n;
     int clear;
 } FFMpvResidualBatch;
+
+/* ---- H.263 deblocking filter (Annex J; H.263+, RV20) over whole pictures ------------------------------------------------------------
+ * What ff_h263_loop_filter (libavcodec/h263.c:135-220) does when the decoder runs it for every macroblock in raster order
+ * (h263dec.c:250-252,281-283, rv10.c:654-655), for n pictures, on `stream`, without synchronising.  The filter of a macroblock writes only
+ * into it and its left / upper neighbours, and no later reconstruction of an H.263 picture reads the picture itself, so running it after
+ * the whole picture has been reconstructed gives the same bytes.  Every macroblock of the macroblock-aligned planes is filtered, the area
+ * past width / height of a custom-size picture included; nothing outside rows [0, 16 * mb_height) x columns [0, 16 * mb_width) (chroma
+ * half of each) is read or written.  The call returns -1 before launching anything when a picture has mb_width / mb_height outside
+ * 1..4096, mb_stride <= mb_width, a linesize below the aligned width, a NULL pointer or a chroma_qscale_table entry above 31, or when two
+ * pictures of the call overlap in memory.  A qscale_table entry outside 1..31 (the decoder stores none) counts as an unfiltered macroblock. */
+typedef struct FFH263LoopFilterPicture {
+    uint8_t *data[3];                   /* s->current_picture.f->data (device) */
+    int linesize, uvlinesize;
+    int mb_width, mb_height, mb_stride;
+    const uint32_t *mb_type;            /* device, s->current_picture.mb_type, indexed mb_x + mb_y * mb_stride; only IS_SKIP is read */
+    const int8_t *qscale_table;         /* device, s->current_picture.qscale_table, same index */
+    uint8_t chroma_qscale_table[32];    /* s->chroma_qscale_table: the default one, or ff_h263_chroma_qscale_table under Annex T */
+} FFH263LoopFilterPicture;
+int ff_h263_loop_filter_batch_cuda(const FFH263LoopFilterPicture *pictures /* host array */, int n_pictures, void *stream);
+
 typedef struct FFMpvPictureWork {
     const FFMpvMCPicture *pictures; int n_pictures;     /* host array: ff_mpv_motion_batch_cuda */
     uint32_t *rejected;                                 /* device uint32, see ff_mpv_motion_batch_cuda */
     const FFMpvResidualBatch *residual; int n_residual; /* host array, run in this order after the motion compensation */
+    const FFH263LoopFilterPicture *loop_filter;         /* host array, NULL / 0: none; ff_h263_loop_filter_batch_cuda after the residual */
+    int n_loop_filter;
 } FFMpvPictureWork;
 int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *work /* host struct */, void *stream);
 
@@ -743,6 +785,10 @@ void ff_h264_pred_init_cuda(H264PredContext *h, int codec_id, const int bit_dept
 void ff_pixblockdsp_init_cuda(PixblockDSPContext *c, unsigned high_bit_depth);
 /* libavcodec/qpeldsp.h:75-77 */
 void ff_qpeldsp_init_cuda(QpelDSPContext *c);
+/* H263DSPContext (libavcodec/h263dsp.c:117-124): h263_h_loop_filter / h263_v_loop_filter as a batch of one through the picture filter's
+ * line arithmetic; host pointers, the 4 x 8 samples the C function reads around src (two before it) staged and written back.  A qscale
+ * outside 0..31, where the C function would read past its strength table, leaves the samples untouched. */
+void ff_h263dsp_init_cuda(H263DSPContext *c);
 /* libavcodec/fft_template.c:152-159, mdct_template.c:58-66 (same shape as ff_fft_init_x86 / ff_mdct_init_x86): called after
  * ff_fft_init / ff_mdct_init filled the context.  fft_permute stays the reference's; the CUDA fft_calc accepts its revtab
  * order, the MDCT slots use the context's own tcos / tsin tables. */

@@ -133,6 +133,12 @@ typedef struct QpelDSPContext {
     qpel_mc_func put_no_rnd_qpel_pixels_tab[2][16];
 } QpelDSPContext;
 
+/* ---- libavcodec/h263dsp.h:26-29 ---- */
+typedef struct H263DSPContext {
+    void (*h263_h_loop_filter)(uint8_t *src, int stride, int qscale);
+    void (*h263_v_loop_filter)(uint8_t *src, int stride, int qscale);
+} H263DSPContext;
+
 /* ---- libavcodec/h264chroma.h:25-30 ---- */
 typedef void (*h264_chroma_mc_func)(uint8_t *dst, uint8_t *src, ptrdiff_t srcStride, int h, int x, int y);
 typedef struct H264ChromaContext {

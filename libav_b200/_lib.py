@@ -97,6 +97,7 @@ PROTOTYPES = {
     "ff_hpel_batch_cuda": (i32, [vp, sz, vp, vp, pd, vp]),
     "ff_mpv_motion_batch_cuda": (i32, [vp, i32, vp, vp]),
     "ff_mpv_flush_pictures_cuda": (i32, [vp, vp]),
+    "ff_h263_loop_filter_batch_cuda": (i32, [vp, i32, vp]),
     "ff_fdct_batch_cuda": (i32, [i32, vp, sz, vp]),
     "ff_fft_batch_cuda": (i32, [i32, i32, vp, sz, vp]),
     "ff_mdct_batch_cuda": (i32, [i32, i32, C.c_double, vp, vp, sz, vp]),
@@ -126,6 +127,7 @@ PROTOTYPES = {
     "ff_hpeldsp_init_cuda": (None, [vp, i32]),
     "ff_h264_pred_init_cuda": (None, [vp, i32, i32, i32]),
     "ff_qpeldsp_init_cuda": (None, [vp]),
+    "ff_h263dsp_init_cuda": (None, [vp]),
     "ff_pixblockdsp_init_cuda": (None, [vp, C.c_uint]),
     "ff_fft_init_cuda": (None, [vp]),
     "ff_mdct_init_cuda": (None, [vp]),

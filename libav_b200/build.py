@@ -7,6 +7,8 @@
   oracle/_ref/libxvidref.so     TEST ONLY: the reference's Xvid IDCT, same conditions
   oracle/_ref/libmpvmcref.so    TEST ONLY: the reference's mpegvideo motion compensation, same conditions
   oracle/_ref/libmpvqref.so     TEST ONLY: the reference's encoder quantisers (plain, trellis, noise reduction), same conditions
+  oracle/_ref/libmpvobmcref.so  TEST ONLY: the reference's H.263 overlapped block motion compensation (apply_obmc), same conditions
+  oracle/_ref/libh263ref.so     TEST ONLY: the reference's H.263 deblocking filter (H263DSPContext, ff_h263_loop_filter), same conditions
 All outputs are in-tree so they travel to the GPU box with the snapshot.
 """
 import glob
@@ -91,6 +93,10 @@ def build_oracle_ref(force=False):
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvmc.mk", "REF=" + REFERENCE])
     # the encoder quantisers (oracle/_ref/libmpvqref.so), linked against libavref.so
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvq.mk", "REF=" + REFERENCE])
+    # the H.263 overlapped block motion compensation (oracle/_ref/libmpvobmcref.so), linked against libavref.so
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvobmc.mk", "REF=" + REFERENCE])
+    # the H.263 deblocking filter (oracle/_ref/libh263ref.so), linked against libavref.so
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "h263.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

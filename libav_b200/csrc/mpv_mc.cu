@@ -1,10 +1,13 @@
 // libav_b200/csrc/mpv_mc.cu -- batched mpegvideo motion compensation (ff_mpv_motion, libavcodec/mpegvideo_motion.c) and the picture flush
 // point of an MPEG-1 / MPEG-2 / H.263 / MPEG-4 decoder back-end.
 //
-// One warp per macroblock record, one lane per destination column (mpv_mc_block.cuh).  Up to MPV_PICS_PER_LAUNCH pictures travel as
+// One warp per macroblock record, one lane per destination column (mpv_mc_block.cuh; OBMC pictures in their own kernel, mpv_obmc.cuh).  Up to MPV_PICS_PER_LAUNCH pictures travel as
 // kernel parameters; a warp finds its picture by scanning their record offsets.  The pictures' checks are all made on the host before
 // anything is launched, so a refused call leaves the destination as it was.
 #include "mpv_mc_block.cuh"
+#include "mpv_obmc.cuh"
+#include "h263_lf.cuh"
+#include <algorithm>
 
 namespace avb {
 
@@ -33,6 +36,33 @@ __global__ void __launch_bounds__(128) mpv_mc_kernel(const __grid_constant__ Mpv
     mpv_mc_lane(P, r, threadIdx.x & 31);
 }
 
+// OBMC pictures (obmc set in a P picture): the same walk, with each record's FFMpvOBMCRecord and put_obmc's weights
+struct MpvObmcLaunch {
+    MpvMcPic pic[MPV_PICS_PER_LAUNCH];
+    const FFMpvMCRecord *recs[MPV_PICS_PER_LAUNCH];
+    const FFMpvOBMCRecord *obmc[MPV_PICS_PER_LAUNCH];
+    unsigned long long start[MPV_PICS_PER_LAUNCH + 1];
+    int n;
+    uint32_t *rejected;
+    uint8_t weights[64];
+};
+
+__global__ void __launch_bounds__(128) mpv_obmc_kernel(const __grid_constant__ MpvObmcLaunch L)
+{
+    const unsigned long long w = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (w >= L.start[L.n]) return;
+    int p = 0;
+    while (p + 1 < L.n && w >= L.start[p + 1]) p++;
+    const MpvMcPic &P = L.pic[p];
+    const FFMpvMCRecord r = L.recs[p][w - L.start[p]];
+    if (mpv_obmc_reject(P, r)) {
+        if ((threadIdx.x & 31) == 0) atomicAdd(L.rejected, 1u);
+        return;
+    }
+    const FFMpvOBMCRecord o = L.obmc[p][w - L.start[p]];
+    mpv_obmc_lane(P, r, o, L.weights, threadIdx.x & 31);
+}
+
 namespace {
 
 int refuse(const char *msg) { set_error_msg("ff_mpv_motion_batch_cuda", msg); return -1; }
@@ -40,12 +70,16 @@ int refuse(const char *msg) { set_error_msg("ff_mpv_motion_batch_cuda", msg); re
 // the frame the picture writes: dest[0] of a bottom field starts one line into it
 const uint8_t *frame_base(const FFMpvMCPicture &q) { return q.dest[0] - (q.picture_structure == 2 ? q.linesize : 0); }
 
+// apply_obmc runs instead of ff_mpv_motion (mpegvideo_motion.c:829-831)
+bool mpv_obmc_picture(const FFMpvMCPicture &q) { return q.obmc && !q.b_picture; }
+
 // the picture-level checks; fills the kernel's view of the picture
 int mpv_picture(const FFMpvMCPicture &q, MpvMcPic &P)
 {
     if (q.out_format == 1) return refuse("H.261 is not supported");
     if (q.out_format != 0 && q.out_format != 2) return refuse("out_format must be 0 (MPEG-1 / MPEG-2) or 2 (H.263 / MPEG-4)");
-    if (q.obmc) return refuse("OBMC is not supported");
+    if (q.obmc && !q.b_picture && (q.out_format != 2 || q.quarter_sample || (q.n_recs && !q.obmc_recs)))
+        return refuse("OBMC is supported in half-sample H.263-family P pictures with obmc_recs only");
     if (q.sprite) return refuse("GMC / sprite pictures are not supported");
     if (q.mspel) return refuse("WMV2 mspel is not supported");
     if (q.lowres) return refuse("lowres is not supported");
@@ -106,24 +140,164 @@ extern "C" int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pics, int n, uint3
         }
     if (!rc) {
         enter();
-        for (int g = 0; g < n && !rc; g += MPV_PICS_PER_LAUNCH) {
+        // the plain pictures, then the OBMC ones in launches of their own; pictures of a call are independent
+        int *order = new int[n], n_plain = 0;
+        for (int i = 0; i < n; i++)
+            if (!mpv_obmc_picture(pics[i])) order[n_plain++] = i;
+        for (int i = 0, k = n_plain; i < n; i++)
+            if (mpv_obmc_picture(pics[i])) order[k++] = i;
+        for (int g = 0; g < n_plain && !rc; g += MPV_PICS_PER_LAUNCH) {
             MpvMcLaunch L;
             memset(&L, 0, sizeof(L));
-            L.n = n - g < MPV_PICS_PER_LAUNCH ? n - g : MPV_PICS_PER_LAUNCH;
+            L.n = n_plain - g < MPV_PICS_PER_LAUNCH ? n_plain - g : MPV_PICS_PER_LAUNCH;
             L.rejected = rejected;
             for (int p = 0; p < L.n; p++) {
-                L.pic[p] = P[g + p];
-                L.recs[p] = pics[g + p].recs;
-                L.start[p + 1] = L.start[p] + pics[g + p].n_recs;
+                L.pic[p] = P[order[g + p]];
+                L.recs[p] = pics[order[g + p]].recs;
+                L.start[p + 1] = L.start[p] + pics[order[g + p]].n_recs;
             }
             const unsigned long long warps = L.start[L.n];
             if (!warps) continue;
             AVB_LAUNCH(mpv_mc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
             rc = check_launch("ff_mpv_motion_batch_cuda");
         }
+        for (int g = n_plain; g < n && !rc; g += MPV_PICS_PER_LAUNCH) {
+            MpvObmcLaunch L;
+            memset(&L, 0, sizeof(L));
+            L.n = n - g < MPV_PICS_PER_LAUNCH ? n - g : MPV_PICS_PER_LAUNCH;
+            L.rejected = rejected;
+            memcpy(L.weights, mpv_obmc_weights, sizeof(L.weights));
+            for (int p = 0; p < L.n; p++) {
+                L.pic[p] = P[order[g + p]];
+                L.recs[p] = pics[order[g + p]].recs;
+                L.obmc[p] = pics[order[g + p]].obmc_recs;
+                L.start[p + 1] = L.start[p] + pics[order[g + p]].n_recs;
+            }
+            const unsigned long long warps = L.start[L.n];
+            if (!warps) continue;
+            AVB_LAUNCH(mpv_obmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
+            rc = check_launch("ff_mpv_motion_batch_cuda");
+        }
+        delete[] order;
     }
     delete[] P;
     return rc;
+}
+
+// ---- the H.263 loop filter over whole pictures (h263_lf.cuh)
+
+namespace avb {
+namespace {
+
+int lf_refuse(const char *msg) { set_error_msg("ff_h263_loop_filter_batch_cuda", msg); return -1; }
+
+// the picture-level checks; fills the kernel's view of the picture
+int h263_lf_picture(const FFH263LoopFilterPicture &q, H263LfPic &P)
+{
+    if (q.mb_width <= 0 || q.mb_height <= 0 || q.mb_width > 4096 || q.mb_height > 4096) return lf_refuse("bad macroblock dimensions");
+    if (q.mb_stride <= q.mb_width) return lf_refuse("mb_stride must exceed mb_width");
+    if (q.linesize < 16 * q.mb_width || q.uvlinesize < 8 * q.mb_width) return lf_refuse("linesize / uvlinesize below the macroblock-aligned width");
+    if (!q.data[0] || !q.data[1] || !q.data[2] || !q.mb_type || !q.qscale_table) return lf_refuse("NULL plane or table");
+    for (int i = 0; i < 32; i++)
+        if (q.chroma_qscale_table[i] > 31) return lf_refuse("chroma_qscale_table entries must be 0..31");
+    P = H263LfPic();
+    for (int i = 0; i < 3; i++) P.data[i] = q.data[i];
+    P.ls[0] = q.linesize; P.ls[1] = q.uvlinesize;
+    P.mb_w = q.mb_width; P.mb_h = q.mb_height; P.mb_stride = q.mb_stride;
+    P.mb_type = q.mb_type; P.qscale = q.qscale_table;
+    for (int i = 0; i < 32; i++) {
+        P.strength[0][i] = h263_lf_strength_tab[i];
+        P.strength[1][i] = h263_lf_strength_tab[q.chroma_qscale_table[i]];
+    }
+    return 0;
+}
+
+// the bytes plane pl of a picture spans (its last row ends at the aligned width)
+void h263_lf_span(const FFH263LoopFilterPicture &q, int pl, uintptr_t &lo, uintptr_t &hi)
+{
+    const int c = pl != 0;
+    lo = (uintptr_t)q.data[pl];
+    hi = lo + (uintptr_t)((16 >> c) * q.mb_height - 1) * (uintptr_t)(c ? q.uvlinesize : q.linesize) + (uintptr_t)((16 >> c) * q.mb_width);
+}
+
+// every check of a call, made before anything is launched
+int h263_lf_check(const FFH263LoopFilterPicture *pics, int n, H263LfPic *P)
+{
+    if (!pics || n < 0) return lf_refuse("NULL pictures or a negative count");
+    for (int i = 0; i < n; i++)
+        if (h263_lf_picture(pics[i], P[i])) return -1;
+    // the planes' spans by start address: a span that begins before the furthest end seen so far overlaps the span reaching that end,
+    // and the first overlap between two pictures in this order is always one of those
+    struct Span { uintptr_t lo, hi; int pic; };
+    Span *sp = new Span[3 * (size_t)n];
+    for (int i = 0; i < n; i++)
+        for (int pl = 0; pl < 3; pl++) { sp[3 * i + pl].pic = i; h263_lf_span(pics[i], pl, sp[3 * i + pl].lo, sp[3 * i + pl].hi); }
+    std::sort(sp, sp + 3 * (size_t)n, [](const Span &a, const Span &b) { return a.lo < b.lo; });
+    int rc = 0;
+    uintptr_t end = 0;
+    int end_pic = -1;
+    for (size_t k = 0; k < 3 * (size_t)n && !rc; k++) {
+        if (sp[k].lo < end && sp[k].pic != end_pic) rc = lf_refuse("two pictures of one call share a frame");
+        if (sp[k].hi > end) { end = sp[k].hi; end_pic = sp[k].pic; }
+    }
+    delete[] sp;
+    return rc;
+}
+
+int h263_lf_run(const FFH263LoopFilterPicture *pics, const H263LfPic *P, int n, cudaStream_t stream)
+{
+    for (int g = 0; g < n; g += H263_LF_PICS_PER_LAUNCH) {
+        const int m = n - g < H263_LF_PICS_PER_LAUNCH ? n - g : H263_LF_PICS_PER_LAUNCH;
+        H263LfLaunch L;
+        memset(&L, 0, sizeof(L));
+        unsigned most = 0;
+        for (int p = 0; p < m; p++) {
+            L.pic[p] = P[g + p];
+            const unsigned t = (unsigned)(2 * pics[g + p].mb_height + 1) * (unsigned)(2 * pics[g + p].mb_width + 1);     // luma tiles
+            most = t > most ? t : most;
+        }
+        AVB_LAUNCH(h263_lf_kernel, dim3((most + 127) / 128, 3 * m), 128, 0, stream)(L);
+        if (check_launch("ff_h263_loop_filter_batch_cuda")) return -1;
+    }
+    return 0;
+}
+
+}  // namespace
+}  // namespace avb
+
+extern "C" int ff_h263_loop_filter_batch_cuda(const FFH263LoopFilterPicture *pics, int n, void *stream)
+{
+    using namespace avb;
+    if (n == 0) return 0;
+    H263LfPic *P = new H263LfPic[n > 0 ? n : 1];
+    int rc = h263_lf_check(pics, n, P);
+    if (!rc) {
+        enter();
+        rc = h263_lf_run(pics, P, n, (cudaStream_t)stream);
+    }
+    delete[] P;
+    return rc;
+}
+
+// the stages of a flush, every check but the motion compensation's (made by its own call, the first stage) already passed
+static int mpv_flush_run(const FFMpvPictureWork *w, const H263LfPic *lf, void *stream)
+{
+    if (w->n_pictures && ff_mpv_motion_batch_cuda(w->pictures, w->n_pictures, w->rejected, stream)) return -1;
+    for (int i = 0; i < w->n_residual; i++) {
+        const FFMpvResidualBatch &b = w->residual[i];
+        if (!b.n) continue;
+        int rc;
+        if (b.dequant < 0)
+            rc = b.transform ? ff_xvid_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+                             : ff_simple_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
+        else
+            rc = b.transform ? ff_mpeg_dequant_xvid_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+                             : ff_mpeg_dequant_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
+        if (rc) return -1;
+    }
+    if (!w->n_loop_filter) return 0;
+    enter();
+    return h263_lf_run(w->loop_filter, lf, w->n_loop_filter, (cudaStream_t)stream);
 }
 
 extern "C" int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *w, void *stream)
@@ -138,18 +312,10 @@ extern "C" int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *w, void *strea
             return -1;
         }
     }
-    if (w->n_pictures && ff_mpv_motion_batch_cuda(w->pictures, w->n_pictures, w->rejected, stream)) return -1;
-    for (int i = 0; i < w->n_residual; i++) {
-        const FFMpvResidualBatch &b = w->residual[i];
-        if (!b.n) continue;
-        int rc;
-        if (b.dequant < 0)
-            rc = b.transform ? ff_xvid_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
-                             : ff_simple_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
-        else
-            rc = b.transform ? ff_mpeg_dequant_xvid_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
-                             : ff_mpeg_dequant_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
-        if (rc) return -1;
-    }
-    return 0;
+    if (w->n_loop_filter < 0 || (w->n_loop_filter && !w->loop_filter)) { set_error_msg(where, "bad loop filter pictures"); return -1; }
+    H263LfPic *lf = new H263LfPic[w->n_loop_filter > 0 ? w->n_loop_filter : 1];
+    int rc = w->n_loop_filter ? h263_lf_check(w->loop_filter, w->n_loop_filter, lf) : 0;
+    if (!rc) rc = mpv_flush_run(w, lf, stream);
+    delete[] lf;
+    return rc;
 }

@@ -62,6 +62,13 @@ class H264DSPContext(C.Structure):          # libavcodec/h264dsp.h:41-117
                 ("startcode_find_candidate", C.CFUNCTYPE(C.c_int, u8p, C.c_int))]
 
 
+h263_loop_filter_func = C.CFUNCTYPE(None, u8p, C.c_int, C.c_int)
+
+
+class H263DSPContext(C.Structure):          # libavcodec/h263dsp.h:26-29
+    _fields_ = [("h263_h_loop_filter", h263_loop_filter_func), ("h263_v_loop_filter", h263_loop_filter_func)]
+
+
 qpel_mc_func = C.CFUNCTYPE(None, u8p, u8p, pd)
 
 
@@ -138,7 +145,7 @@ class FFMpvMCPicture(C.Structure):
                 ("h_edge_pos", C.c_int), ("v_edge_pos", C.c_int), ("out_format", C.c_int), ("picture_structure", C.c_int),
                 ("first_field", C.c_int), ("b_picture", C.c_int), ("no_rounding", C.c_int), ("quarter_sample", C.c_int),
                 ("workaround_bugs", C.c_int), ("chroma_format", C.c_int), ("obmc", C.c_int), ("sprite", C.c_int), ("mspel", C.c_int),
-                ("lowres", C.c_int), ("recs", C.c_void_p), ("n_recs", C.c_size_t)]
+                ("lowres", C.c_int), ("recs", C.c_void_p), ("n_recs", C.c_size_t), ("obmc_recs", C.c_void_p)]
 
 
 class FFMpvResidualBatch(C.Structure):
@@ -148,10 +155,16 @@ class FFMpvResidualBatch(C.Structure):
                 ("clear", C.c_int)]
 
 
+class FFH263LoopFilterPicture(C.Structure):
+    """include/avdsp_b200.h FFH263LoopFilterPicture (host struct holding device pointers): ff_h263_loop_filter_batch_cuda"""
+    _fields_ = [("data", C.c_void_p * 3), ("linesize", C.c_int), ("uvlinesize", C.c_int), ("mb_width", C.c_int), ("mb_height", C.c_int),
+                ("mb_stride", C.c_int), ("mb_type", C.c_void_p), ("qscale_table", C.c_void_p), ("chroma_qscale_table", C.c_uint8 * 32)]
+
+
 class FFMpvPictureWork(C.Structure):
     """include/avdsp_b200.h FFMpvPictureWork (host struct): ff_mpv_flush_pictures_cuda"""
     _fields_ = [("pictures", C.c_void_p), ("n_pictures", C.c_int), ("rejected", C.c_void_p),
-                ("residual", C.c_void_p), ("n_residual", C.c_int)]
+                ("residual", C.c_void_p), ("n_residual", C.c_int), ("loop_filter", C.c_void_p), ("n_loop_filter", C.c_int)]
 
 
 class FFMECmpEncState(C.Structure):
