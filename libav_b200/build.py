@@ -81,22 +81,13 @@ def build_oracle_port(force=False):
 
 
 def build_oracle_ref(force=False):
-    """Compile the reference's own C sources (read in place) with oracle/refbuild/Makefile."""
+    """Compile the reference's own C sources (read in place) with oracle/refbuild/Makefile: libavref.so, its timing-only SIMD
+    flavour and the satellite libraries of single features, all in one make run."""
     if not os.path.isdir(REFERENCE):
         return ORACLE_REF if os.path.exists(ORACLE_REF) else None
     if force:
         shutil.rmtree(os.path.join(ROOT, "oracle", "_ref"), ignore_errors=True)
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "REF=" + REFERENCE])
-    # the Xvid IDCT (oracle/_ref/libxvidref.so), linked against libavref.so
-    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "xvid.mk", "REF=" + REFERENCE])
-    # the mpegvideo motion compensation (oracle/_ref/libmpvmcref.so), linked against libavref.so
-    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvmc.mk", "REF=" + REFERENCE])
-    # the encoder quantisers (oracle/_ref/libmpvqref.so), linked against libavref.so
-    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvq.mk", "REF=" + REFERENCE])
-    # the H.263 overlapped block motion compensation (oracle/_ref/libmpvobmcref.so), linked against libavref.so
-    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvobmc.mk", "REF=" + REFERENCE])
-    # the H.263 deblocking filter (oracle/_ref/libh263ref.so), linked against libavref.so
-    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "h263.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

@@ -5,6 +5,7 @@ __graft_entry__.smoke() and bench.py's CPU legs.
   ref()   oracle/_ref/libavref.so    ref_*  the unmodified reference (built where /root/reference exists;
                                             the prebuilt .so travels to the GPU box)
 Both expose the prototypes of oracle/oracle_api.h through the same attribute names without prefix.
+ref_lib(name) loads one satellite library of the reference, oracle/_ref/lib<name>ref.so; its callers set the prototypes they use.
 """
 import ctypes as C
 import os
@@ -143,6 +144,16 @@ def ref():
     if "ref" not in _cache:
         _cache["ref"] = Oracle(REF_PATH, "ref_") if os.path.exists(REF_PATH) else None
     return _cache["ref"]
+
+
+def ref_lib(name):
+    """The satellite library oracle/_ref/lib<name>ref.so (one feature of the unmodified reference, linked against libavref.so), or None
+    when it has not been built."""
+    key = "lib" + name
+    if key not in _cache:
+        path = os.path.join(_HERE, "_ref", "lib%sref.so" % name)
+        _cache[key] = C.CDLL(path) if os.path.exists(path) else None
+    return _cache[key]
 
 
 def ref_simd():

@@ -2,7 +2,7 @@
  * oracle/refbuild/refapi_h263.c -- TEST INFRASTRUCTURE, NOT PRODUCT.
  *
  * The reference's H.263 deblocking filter (libavcodec/h263dsp.c and the per-macroblock driver ff_h263_loop_filter of
- * libavcodec/h263.c, both compiled UNMODIFIED by h263.mk into oracle/_ref/libh263ref.so next to libavref.so).  No arithmetic of its own.
+ * libavcodec/h263.c, both compiled UNMODIFIED by Makefile into oracle/_ref/libh263ref.so next to libavref.so).  No arithmetic of its own.
  *
  * ref_h263_loop_filter_picture() runs ff_h263_loop_filter for every macroblock of one picture in raster order, as h263dec.c decode_slice
  * (:250-252, :281-283) and rv10.c (:654-655) do after each ff_mpv_reconstruct_mb: s->dest as ff_init_block_index / ff_update_block_index

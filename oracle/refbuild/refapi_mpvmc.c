@@ -1,9 +1,9 @@
 /*
  * oracle/refbuild/refapi_mpvmc.c -- TEST INFRASTRUCTURE, NOT PRODUCT.
  *
- * The reference's motion compensation for the mpegvideo decoders (libavcodec/mpegvideo_motion.c, compiled UNMODIFIED by mpvmc.mk into
+ * The reference's motion compensation for the mpegvideo decoders (libavcodec/mpegvideo_motion.c, compiled UNMODIFIED by Makefile into
  * oracle/_ref/libmpvmcref.so next to libavref.so).  libavref.so exports an aborting stand-in under the name ff_mpv_motion
- * (refapi_mpv_stubs.c); mpvmc.mk compiles the real function as ref_real_mpv_motion, so the two never meet.
+ * (refapi_mpv_stubs.c); Makefile compiles the real function as ref_real_mpv_motion, so the two never meet.
  *
  * ref_mpvmc_picture() builds an MpegEncContext the way ff_mpv_frame_start() and mpeg_field_start() leave it for one picture (current /
  * last / next picture planes, doubled linesizes in a field picture, the DSP tables, an edge emulation buffer) and runs, per record, what

@@ -1,7 +1,7 @@
 /*
  * oracle/refbuild/refapi_mpvobmc.c -- TEST INFRASTRUCTURE, NOT PRODUCT.
  *
- * The reference's overlapped block motion compensation (apply_obmc in libavcodec/mpegvideo_motion.c, compiled UNMODIFIED by mpvobmc.mk
+ * The reference's overlapped block motion compensation (apply_obmc in libavcodec/mpegvideo_motion.c, compiled UNMODIFIED by Makefile
  * into oracle/_ref/libmpvobmcref.so next to libavref.so).  Like refapi_mpvmc.c, the real ff_mpv_motion is compiled under the name
  * ref_real_mpv_motion so that it never meets the aborting stand-in libavref.so exports.  No arithmetic of its own.
  */

@@ -3,7 +3,7 @@
  *
  * The reference's encoder quantisers.  dct_quantize_trellis_c, denoise_dct_c, clip_coeffs and dct_single_coeff_elimination are static in
  * libavcodec/mpegvideo_enc.c, so this unit #includes that file (UNMODIFIED, read in place) and exports only the ref_mpvq_* wrappers below;
- * mpvq.mk compiles it with hidden visibility, so the file's own external names stay inside oracle/_ref/libmpvqref.so, and links it against
+ * Makefile compiles it with hidden visibility, so the file's own external names stay inside oracle/_ref/libmpvqref.so, and links it against
  * libavref.so for everything else (the FDCTs, av_log, the encoder's stubs).
  *
  * ref_mpvq_batch() runs, for every record, what encode_mb_internal (mpegvideo_enc.c:2263-2303) runs for one block on one context:

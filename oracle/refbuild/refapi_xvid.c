@@ -1,7 +1,7 @@
 /*
  * oracle/refbuild/refapi_xvid.c -- TEST INFRASTRUCTURE, NOT PRODUCT.
  *
- * The reference's Xvid IDCT (libavcodec/xvididct.c, compiled unmodified by xvid.mk into oracle/_ref/libxvidref.so next to
+ * The reference's Xvid IDCT (libavcodec/xvididct.c, compiled unmodified by Makefile into oracle/_ref/libxvidref.so next to
  * libavref.so) reached the way the MPEG-4 decoder reaches it: ff_xvid_idct_init() fills an IDCTDSPContext and every call goes
  * through that table.  ff_idctdsp_init() runs first, because xvid_idct_put / _add call the global ff_put_pixels_clamped /
  * ff_add_pixels_clamped, which only it sets.  No arithmetic of its own.

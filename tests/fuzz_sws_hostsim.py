@@ -1,23 +1,19 @@
 """TEST INFRASTRUCTURE (not collected by pytest): randomised differential run of the scaler's whole-frame host call -- libav_b200/csrc/swscale.cu compiled
-for the host (tests/hostsim/, build it by running tests/test_hostsim_sws_frames_cpu.py once) -- against the compiled reference (oracle/_ref).  Random
+for the host (tests/hostsim/, built by tests/hostsim_build.py) -- against the compiled reference (oracle/_ref).  Random
 source / destination format, geometry and flags; every request the product accepts must give the reference's picture bytes.
 usage: python tests/fuzz_sws_hostsim.py [seed [requests]]        (round 2: seeds 1-12 and 21-23, ~18000 requests, ~14000 accepted; two findings, both fixed: slices into a gray8 destination, bgr24 -> gray8 at the same size)"""
 import sys, os
 HERE = os.path.dirname(os.path.abspath(__file__)); sys.path.insert(0, HERE); sys.path.insert(0, os.path.dirname(HERE))
 import numpy as np, ctypes as C, random
 from oracle import loader
+import hostsim_build
 import test_hostsim_sws_frames_cpu as H
 import test_sws_plan_cpu as P
 import test_sws_gray_src as G
 import test_sws_pal8_src as PAL
 from libav_b200 import synth
 refo = loader.ref()
-lib = C.CDLL(os.path.join(HERE, 'hostsim', 'libslots_hostsim.so'))
-lib.avb200_last_error.restype = C.c_char_p
-lib.sws_getContext_cuda.restype = C.c_void_p
-lib.sws_getContext_cuda.argtypes = [C.c_int] * 7 + [C.c_void_p] * 3
-lib.sws_freeContext_cuda.argtypes = [C.c_void_p]
-lib.sws_scale_cuda.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+lib = hostsim_build.load()
 SRCS = [0,4,5,6,7,31,12,13,14,32,33,8,11,23,24,1,15,2,3,25,26,27,28,62,61,64,63,47,48,66,70,72,68,49,51]
 DSTS = [0,4,5,6,7,31,12,13,14,32,2,3,25,26,27,28,1,15,23,24,8,37,36,41,43,54,57,35,34,60,59,62,64,66,68,61,63,72,70]
 SUB = {0:(1,1),4:(1,0),5:(0,0),6:(2,2),7:(2,0),31:(0,1),12:(1,1),13:(1,0),14:(0,0),32:(0,1),33:(1,1)}

@@ -1,18 +1,16 @@
 """Pictures for the H.263 deblocking filter tests (tests/test_h263_cpu.py, tests/test_gpu_h263.py), and the ways of running them: the
 reference's serial driver (ff_h263_loop_filter per macroblock in raster order, oracle/_ref/libh263ref.so), its two-pass plain-C
-restatement (oracle/port/orc_h263.c), the product compiled for the host (tests/hostsim/h263_hostsim.cpp) and the product on the GPU.
+restatement (oracle/port/orc_h263.c), the product compiled for the host (tests/hostsim/) and the product on the GPU.
 Every plane buffer holds random bytes, its padding included: two rows above and below the macroblock-aligned plane and columns to the
 right of it, so a kernel that writes outside the plane gives a different buffer."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
+from oracle import loader
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-H263_REF = os.path.join(ROOT, "oracle", "_ref", "libh263ref.so")
-SIM_LIB = os.path.join(HERE, "hostsim", "libh263_hostsim.so")
 MB_TYPE_SKIP = 1 << 11
 PAD_ROWS = 2
 DEFAULT_CHROMA_QSCALE = np.arange(32, dtype=np.uint8)              # ff_default_chroma_qscale_table (mpegvideodata.c): the identity
@@ -69,16 +67,15 @@ def _bind(fn):
 
 def ref_lib():
     """the reference's serial driver (ref_h263_loop_filter_picture), or None where oracle/_ref was not built"""
-    if not os.path.exists(H263_REF):
+    lib = loader.ref_lib("h263")
+    if lib is None:
         return None
-    lib = C.CDLL(H263_REF)
     lib.picture = _bind(lib.ref_h263_loop_filter_picture)
     return lib
 
 
 class _Port:
     def __init__(self):
-        from oracle import loader
         lib = loader.port().lib
         self.picture = _bind(lib.orc_h263_loop_filter_picture)
         self.h_loop_filter, self.v_loop_filter = lib.orc_h263_h_loop_filter, lib.orc_h263_v_loop_filter
@@ -103,30 +100,6 @@ def run_serial(lib, pic):
     return b
 
 
-def sim_lib():
-    """tests/hostsim/h263_hostsim.cpp built into its own library (under a temporary name, then renamed into place)"""
-    hs = os.path.join(HERE, "hostsim")
-    csrc = os.path.join(ROOT, "libav_b200", "csrc")
-    src = os.path.join(hs, "h263_hostsim.cpp")
-    deps = [src, os.path.join(hs, "mpv_mc_hostsim.cpp"), os.path.join(hs, "shim", "cuda_runtime.h"), os.path.join(csrc, "mpv_mc.cu"),
-            os.path.join(csrc, "mpv_mc_block.cuh"), os.path.join(csrc, "h263_lf.cuh"), os.path.join(csrc, "common.cuh"),
-            os.path.join(ROOT, "include", "avdsp_b200.h")]
-    if not os.path.exists(SIM_LIB) or any(os.path.getmtime(d) > os.path.getmtime(SIM_LIB) for d in deps):
-        tmp = "%s.%d.tmp" % (SIM_LIB, os.getpid())
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-DAVB_HOSTSIM", "-I", os.path.join(hs, "shim"), "-I", csrc,
-                        "-Wno-unknown-pragmas", "-Wl,--no-undefined", "-o", tmp, src], check=True)
-        os.replace(tmp, SIM_LIB)
-    lib = C.CDLL(SIM_LIB)
-    lib.ff_h263_loop_filter_batch_cuda.restype = C.c_int
-    lib.ff_h263_loop_filter_batch_cuda.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    lib.ff_mpv_flush_pictures_cuda.restype = C.c_int
-    lib.ff_mpv_flush_pictures_cuda.argtypes = [C.c_void_p, C.c_void_p]
-    lib.hostsim_h263_slot.restype = C.c_int
-    lib.hostsim_h263_slot.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int]
-    lib.hostsim_last_error.restype = C.c_char_p
-    return lib
-
-
 def host_structs(pics, bufs):
     """an FFH263LoopFilterPicture array over host buffers `bufs` (one list of three planes per picture)"""
     from libav_b200 import tables
@@ -143,7 +116,7 @@ def run_sim(lib, pics):
     bufs = [[a.copy() for a in pic.bufs] for pic in pics]
     arr = host_structs(pics, bufs)
     rc = lib.ff_h263_loop_filter_batch_cuda(C.cast(arr, C.c_void_p), len(pics), None)
-    assert rc == 0, lib.hostsim_last_error()
+    assert rc == 0, lib.avb200_last_error()
     return bufs
 
 

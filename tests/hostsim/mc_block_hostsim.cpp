@@ -6,20 +6,10 @@
 // (shuffle scan, offset search, component votes) is stated here as plain loops; `votes` chooses how the need_* flags are formed:
 // 0 = every component always, 1 = exactly what the block's position uses (the two extremes the warp vote lies between).
 #include "shim/cuda_runtime.h"
-#include <string>
-uint3 threadIdx, blockIdx;
-dim3 blockDim, gridDim;
 #include "h264_mc_block.cuh"
 #include "../../include/avdsp_b200.h"
 // the register-resident residual kernel (one lane per block, lanes never communicate): compiled unchanged, a launch = its body once per thread
 #include "../../libav_b200/csrc/h264_residual.cu"
-
-namespace avb {
-static std::string g_err;
-void set_error_msg(const char *where, const char *msg) { if (g_err.empty()) g_err = std::string(where) + ": " + msg; }
-void set_error(const char *where, cudaError_t) { set_error_msg(where, "hostsim error"); }
-int check_launch(const char *) { return 0; }
-}
 
 extern "C" int hostsim_h264_residual(const FFH264ResidualMB *mbs, size_t n, int16_t *coeffs, size_t coeff_stride, const uint8_t *nnzc,
                                      uint8_t *luma, uint8_t *cb, uint8_t *cr, int ls, int uvls)

@@ -19,6 +19,7 @@
 #define __forceinline__ inline
 #define __launch_bounds__(...)
 #define __shared__
+#define __grid_constant__
 #define __align__(n) __attribute__((aligned(n)))
 
 typedef int cudaError_t;
@@ -101,6 +102,7 @@ static inline unsigned __byte_perm(unsigned a, unsigned b, unsigned sel)
     return r;
 }
 static inline int atomicMin(int *p, int v) { const int old = *p; if (v < old) *p = v; return old; }      /* threads run one after the other here */
+static inline unsigned atomicAdd(unsigned *p, unsigned v) { const unsigned old = *p; *p = old + v; return old; }
 static inline int __mulhi(int a, int b) { return (int)(((int64_t)a * b) >> 32); }
 static inline size_t __cvta_generic_to_shared(const void *p) { return (size_t)p; }
 

@@ -5,52 +5,7 @@
 // that the CPU suite can drive the H.264 slots exactly like tests/test_gpu_slots.py drives them on the GPU and compare them
 // with the oracle.  This library is never loaded by the product and never measured; it exists because the GPU box is not
 // always at hand while the slot code changes.  Slots that route through the batched kernels (FDCT, me_cmp, hpel, MPEG-4 qpel,
-// pixblock, weight) need warps and shared memory and are not simulated: their launchers fail loudly here.
+// pixblock, weight) need warps and shared memory and are not simulated: their launchers fail loudly (runtime_hostsim.cpp).
 #include "shim/cuda_runtime.h"
-#include <mutex>
-#include <string>
-
-uint3 threadIdx, blockIdx;
-dim3 blockDim, gridDim;
-
 #include "../../libav_b200/csrc/slots.cu"
 #include "../../libav_b200/csrc/fdct10.cu"
-
-namespace avb {
-static std::string g_err;
-void set_error_msg(const char *where, const char *msg) { if (g_err.empty()) g_err = std::string(where) + ": " + msg; }
-void set_error(const char *where, cudaError_t) { set_error_msg(where, "hostsim error"); }
-int check_launch(const char *) { return 0; }
-void enter() {}
-int sm_count() { return 148; }
-// the general scaler is forced onto its two-pass path here: the tile kernels synchronise their threads (swscale_hostsim.cpp)
-int tuning(const char *key) { return !strcmp(key, "sws_general_variant") ? 1 : 0; }
-
-static Scratch g_scratch;
-static std::recursive_mutex g_mu;
-Scratch &scratch() { return g_scratch; }
-std::recursive_mutex &scratch_mutex() { return g_mu; }
-// real device / pinned allocations come back uninitialised: poison them so that a kernel reading bytes nobody staged cannot pass by luck
-static void *grow(void *&p, size_t &n, size_t bytes) { if (n < bytes) { free(p); p = malloc(bytes); memset(p, 0xA7, bytes); n = bytes; } return p; }
-void *Scratch::dev(int slot, size_t bytes) { void *p = grow(d_[slot], dn_[slot], bytes); memset(p, 0xA7, bytes); return p; }      // (every call: contents are undefined)
-void *Scratch::pinned(size_t bytes) { return grow(h_, hn_, bytes); }
-void *Scratch::pinned2(size_t bytes) { void *p = grow(h2_, h2n_, bytes); memset(p, 0x5B, bytes); return p; }
-cudaStream_t *Scratch::streams() { return st_; }
-}  // namespace avb
-
-extern "C" {
-const char *avb200_last_error(void) { return avb::g_err.c_str(); }
-void avb200_clear_error(void) { avb::g_err.clear(); }
-#define NOT_SIMULATED(name) { avb::set_error_msg(name, "batched kernel: not simulated on the host"); return -1; }
-int ff_me_cmp_batch_cuda(int, int, int, const uint8_t *, const uint8_t *, ptrdiff_t, int, const FFMECmpRecord *, size_t, int32_t *, void *) NOT_SIMULATED("ff_me_cmp_batch_cuda")
-int ff_hpel_batch_cuda(const FFHpelRecord *, size_t, uint8_t *, const uint8_t *, ptrdiff_t, void *) NOT_SIMULATED("ff_hpel_batch_cuda")
-// the 8-bit transforms are warp kernels (me_cmp.cu, not simulated); the 10-bit ones are thread-per-block (fdct10.cu, included below)
-int ff_fdct_batch_cuda(int which, int16_t *blocks, size_t n, void *stream)
-{
-    if (which == 4 || which == 5) return avb::fdct10_launch(which, blocks, n, (cudaStream_t)stream);
-    NOT_SIMULATED("ff_fdct_batch_cuda")
-}
-int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *, size_t, uint8_t *, const uint8_t *, ptrdiff_t, void *) NOT_SIMULATED("ff_mpeg4_qpel_batch_cuda")
-int ff_pixblock_fdct_batch_cuda(int, const uint8_t *, const uint8_t *, const uint32_t *, const uint32_t *, ptrdiff_t, int16_t *, size_t, void *) NOT_SIMULATED("ff_pixblock_fdct_batch_cuda")
-int ff_h264_weight_batch_cuda(const FFH264WeightRecord *, size_t, uint8_t *, const uint8_t *, int, void *) NOT_SIMULATED("ff_h264_weight_batch_cuda")
-}

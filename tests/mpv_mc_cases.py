@@ -3,15 +3,10 @@ four ways of running them: the reference's own ff_mpv_motion through oracle/_ref
 (oracle/port/orc_mpvmc.c), the product compiled for the host (tests/hostsim/mpv_mc_hostsim.cpp) and the product on the GPU.  Every plane buffer, its padding included, holds random bytes, so a kernel
 that clamps where the reference reads directly, or writes outside its macroblock, gives a different buffer."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-MPVMC_REF = os.path.join(ROOT, "oracle", "_ref", "libmpvmcref.so")
-SIM_LIB = os.path.join(HERE, "hostsim", "libmpvmc_hostsim.so")
+from oracle import loader
 
 REC = np.dtype([("mb_x", "<u2"), ("mb_y", "<u2"), ("mv_dir", "u1"), ("mv_type", "u1"), ("field_select", "u1", (2, 2)),
                 ("mv", "<i2", (2, 4, 2)), ("pad", "u1", (2,))])
@@ -135,9 +130,9 @@ def make_records(rng, pic, n=None, far=0.1, edge=0.35, types=None):
 
 def ref_lib():
     """the reference (ref_mpvmc_picture), or None where oracle/_ref was not built"""
-    if not os.path.exists(MPVMC_REF):
+    lib = loader.ref_lib("mpvmc")
+    if lib is None:
         return None
-    lib = C.CDLL(MPVMC_REF)
     lib.picture = lib.ref_mpvmc_picture
     lib.picture.restype = C.c_int
     lib.picture.argtypes = [C.c_void_p] * 5 + [C.c_void_p, C.c_size_t]
@@ -149,7 +144,6 @@ class _Port:
     """the plain-C restatement (orc_mpvmc_picture in oracle/liboracle_port.so), called like the reference"""
 
     def __init__(self):
-        from oracle import loader
         self.picture = loader.port().lib.orc_mpvmc_picture
         self.picture.restype = C.c_int
         self.picture.argtypes = [C.c_void_p] * 5 + [C.c_void_p, C.c_size_t]
@@ -179,25 +173,6 @@ def run_ref(lib, pic, frame=None):
     return f
 
 
-def sim_lib():
-    """tests/hostsim/mpv_mc_hostsim.cpp built into its own library (under a temporary name, then renamed into place)"""
-    hs = os.path.join(HERE, "hostsim")
-    csrc = os.path.join(ROOT, "libav_b200", "csrc")
-    src = os.path.join(hs, "mpv_mc_hostsim.cpp")
-    deps = [src, os.path.join(hs, "shim", "cuda_runtime.h"), os.path.join(csrc, "mpv_mc.cu"), os.path.join(csrc, "mpv_mc_block.cuh"),
-            os.path.join(csrc, "common.cuh"), os.path.join(ROOT, "include", "avdsp_b200.h")]
-    if not os.path.exists(SIM_LIB) or any(os.path.getmtime(d) > os.path.getmtime(SIM_LIB) for d in deps):
-        tmp = "%s.%d.tmp" % (SIM_LIB, os.getpid())
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-DAVB_HOSTSIM", "-I", os.path.join(hs, "shim"), "-I", csrc,
-                        "-Wno-unknown-pragmas", "-Wl,--no-undefined", "-o", tmp, src], check=True)
-        os.replace(tmp, SIM_LIB)
-    lib = C.CDLL(SIM_LIB)
-    lib.ff_mpv_motion_batch_cuda.restype = C.c_int
-    lib.ff_mpv_motion_batch_cuda.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.hostsim_last_error.restype = C.c_char_p
-    return lib
-
-
 def picture_struct(pic, dest, cur, last, nxt, recs_ptr, n_recs):
     """FFMpvMCPicture from plane base pointers (host or device addresses)"""
     from libav_b200 import tables
@@ -222,7 +197,7 @@ def run_sim(lib, pics):
         arr[i] = picture_struct(pic, base, base, [a.ctypes.data for a in pic.last], [a.ctypes.data for a in pic.next], recs[i].ctypes.data, len(recs[i]))
     rej = np.zeros(1, np.uint32)
     rc = lib.ff_mpv_motion_batch_cuda(C.cast(arr, C.c_void_p), len(pics), rej.ctypes.data, None)
-    assert rc == 0, lib.hostsim_last_error()
+    assert rc == 0, lib.avb200_last_error()
     return frames, int(rej[0])
 
 
@@ -280,9 +255,9 @@ def residual_batch(checker, pics, pi, pl, tr, dq, mode, offs, stride, clear, see
 
 def xvid_checker():
     """the Xvid IDCT checker: the compiled reference where it was built, else the port"""
-    from test_xvid_idct import XVID_REF, Xvid
-    from oracle import loader
-    return Xvid(C.CDLL(XVID_REF), "ref_") if os.path.exists(XVID_REF) else Xvid(loader.port().lib, "orc_")
+    from test_xvid_idct import Xvid
+    lib = loader.ref_lib("xvid")
+    return Xvid(lib, "ref_") if lib else Xvid(loader.port().lib, "orc_")
 
 
 def apply_residual(checker, xv, frames, batches):
@@ -290,7 +265,6 @@ def apply_residual(checker, xv, frames, batches):
     last_index < 0), then idct_put / idct_add through the simple or the Xvid IDCT oracle.  Returns, per batch, the mask of the blocks the
     call consumes (what `clear` zeroes)."""
     from test_gpu_mpv import INTER, oracle_dequant
-    from oracle import loader
     keeps = []
     for b in batches:
         f, n = frames[b["pi"]][b["pl"]], len(b["off"])

@@ -1,17 +1,14 @@
 """Pictures and records for the H.263 overlapped block motion compensation tests (tests/test_mpv_obmc_cpu.py, tests/test_gpu_mpv_obmc.py):
 H.263 half-sample P pictures of tests/mpv_mc_cases.py with one FFMpvOBMCRecord per record, and the ways of running them -- the reference's
 apply_obmc through the real ff_mpv_motion (oracle/_ref/libmpvobmcref.so), its plain-C restatement (oracle/port/orc_mpvobmc.c), the product
-compiled for the host (tests/hostsim/h263_hostsim.cpp) and the product on the GPU."""
+compiled for the host (tests/hostsim/mpv_mc_hostsim.cpp) and the product on the GPU."""
 import ctypes as C
-import os
 
 import numpy as np
 
+from oracle import loader
 import mpv_mc_cases as M
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-OBMC_REF = os.path.join(ROOT, "oracle", "_ref", "libmpvobmcref.so")
 OBMC = np.dtype([("mv", "<i2", (4, 2)), ("top", "<i2", (2, 2)), ("left", "<i2", (2, 2)), ("right", "<i2", (2, 2)),
                  ("mb_type_top", "<u4"), ("mb_type_left", "<u4"), ("mb_type_right", "<u4")])
 assert OBMC.itemsize == 52
@@ -69,16 +66,15 @@ def _bind(fn):
 
 
 def ref_lib():
-    if not os.path.exists(OBMC_REF):
+    lib = loader.ref_lib("mpvobmc")
+    if lib is None:
         return None
-    lib = C.CDLL(OBMC_REF)
     lib.picture = _bind(lib.ref_mpvmc_obmc_picture)
     return lib
 
 
 class _Port:
     def __init__(self):
-        from oracle import loader
         self.picture = _bind(loader.port().lib.orc_mpvobmc_picture)
 
 
@@ -121,5 +117,5 @@ def run_sim(lib, pics):
                   [[a.ctypes.data for a in p.last] for p in pics], [[a.ctypes.data for a in p.next] for p in pics])
     rej = np.zeros(1, np.uint32)
     rc = lib.ff_mpv_motion_batch_cuda(C.cast(arr, C.c_void_p), len(pics), rej.ctypes.data, None)
-    assert rc == 0, lib.hostsim_last_error()
+    assert rc == 0, lib.avb200_last_error()
     return frames, int(rej[0])

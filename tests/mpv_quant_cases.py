@@ -3,17 +3,11 @@ length tables, blocks fetched from pixel planes, per-block records, and the runn
 ref_mpvq_batch: mpegvideo_enc.c's own static quantisers on a context), its plain-C restatement (oracle/port/orc_mpvq.c), the product compiled
 for the host (tests/hostsim/mpv_quant_hostsim.cpp) and the product on the GPU."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
+from oracle import loader
 from oracle.loader import OrcEncState
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-MPVQ_REF = os.path.join(ROOT, "oracle", "_ref", "libmpvqref.so")
-SIM_LIB = os.path.join(HERE, "hostsim", "libmpvq_hostsim.so")
 
 REC = np.dtype([("qscale", np.uint8), ("intra", np.uint8), ("dc_scale", np.uint8), ("chroma", np.uint8), ("lambda2", np.uint32)])
 FMT_MPEG1, FMT_H261, FMT_H263, FMT_MJPEG = 0, 1, 2, 3
@@ -209,16 +203,15 @@ class Oracle:
 
 def ref_oracle():
     """the reference's quantisers, or None where oracle/_ref was not built"""
-    if not os.path.exists(MPVQ_REF):
+    lib = loader.ref_lib("mpvq")
+    if lib is None:
         return None
-    lib = C.CDLL(MPVQ_REF)
     o = Oracle(lib.ref_mpvq_batch, "ref")
     o.lib = lib
     return o
 
 
 def port_oracle():
-    from oracle import loader
     return Oracle(loader.port().lib.orc_mpvq_batch, "port")
 
 
@@ -229,42 +222,10 @@ def checker():
 
 def matrices_checker():
     """the ff_convert_matrix the q matrices come from: the reference's where it was built, else its restatement"""
-    from oracle import loader
     return loader.ref() or loader.port()
 
 
 # ------------------------------------------------------------------------------------------------------------------------------ product
-
-def sim_lib():
-    """the product's mpv_quant.cu as host C++ (tests/hostsim/mpv_quant_hostsim.cpp) with the shim runtime and the shared VLC cache, built into
-    its own library under a temporary name and renamed into place"""
-    hs = os.path.join(HERE, "hostsim")
-    csrc = os.path.join(ROOT, "libav_b200", "csrc")
-    srcs = [os.path.join(hs, f) for f in ("slots_hostsim.cpp", "slots_hbd_hostsim.cpp", "me_cmp_enc_hostsim.cpp", "mpv_quant_hostsim.cpp")]
-    deps = srcs + [os.path.join(hs, "shim", "cuda_runtime.h")] + \
-        [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cu", ".cuh", ".h"))] + \
-        [os.path.join(ROOT, "include", f) for f in ("avdsp_b200.h", "avdsp_b200_tables.h")]
-    if not os.path.exists(SIM_LIB) or any(os.path.getmtime(d) > os.path.getmtime(SIM_LIB) for d in deps):
-        tmp = "%s.%d.tmp" % (SIM_LIB, os.getpid())
-        try:
-            subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-DAVB_HOSTSIM", "-I", os.path.join(hs, "shim"), "-I", csrc,
-                            "-Wno-unknown-pragmas", "-Wl,--no-undefined", "-o", tmp] + srcs, check=True)
-            os.replace(tmp, SIM_LIB)
-        finally:
-            if os.path.exists(tmp):
-                os.remove(tmp)
-    lib = C.CDLL(SIM_LIB)
-    bind(lib)
-    return lib
-
-
-def bind(lib):
-    from libav_b200 import _lib
-    for name in ("ff_mpv_quant_state_cuda", "ff_mpv_quant_state_free_cuda", "ff_mpv_dct_quantize_batch_cuda", "ff_mpv_quantize_init_cuda",
-                 "ff_mpv_quantize_uninit_cuda", "avb200_last_error", "avb200_clear_error"):
-        restype, argtypes = _lib.PROTOTYPES[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = restype, argtypes
-
 
 def nr_struct(offset_ptr, sum_ptr, count_ptr):
     from libav_b200 import tables
@@ -303,7 +264,6 @@ def undefined_blocks(st, vlc, trellis, recs, blocks, nr=None):
     beats the initial best score): the port run with two different table fillings disagrees on exactly those"""
     if not trellis:
         return np.zeros(len(recs), bool)
-    from oracle import loader
     fill = loader.port().lib.orc_mpvq_set_table_fill
     port = port_oracle()
     out = []

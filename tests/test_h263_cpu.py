@@ -1,5 +1,5 @@
 """CPU: the H.263 deblocking filter.  The product's picture filter (libav_b200/csrc/h263_lf.cuh) compiled for the host
-(tests/hostsim/h263_hostsim.cpp) and its two-pass plain-C restatement (oracle/port/orc_h263.c) against the reference's serial driver --
+(tests/hostsim/mpv_mc_hostsim.cpp) and its two-pass plain-C restatement (oracle/port/orc_h263.c) against the reference's serial driver --
 ff_h263_loop_filter for every macroblock in raster order, libavcodec/h263.c with h263dsp.c, oracle/_ref/libh263ref.so -- whole buffers
 byte for byte, padding included: random pictures with random skip flags and qscale 1..31, mostly and wholly skipped pictures, both
 chroma qscale tables, 1 x N, N x 1 and 1 x 1 macroblock pictures, several pictures per call.  The port matching the serial driver is the
@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 import h263_cases as H
+import hostsim_build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -27,9 +28,9 @@ def lfref(built):
     return lib
 
 
-@pytest.fixture(scope="module")
+@pytest.fixture
 def lfsim(built):
-    return H.sim_lib()
+    return hostsim_build.fresh()
 
 
 @pytest.fixture(scope="module")
@@ -129,9 +130,9 @@ def test_refusals_change_nothing(lfsim):
         bufs = [[a.copy() for a in p.bufs] for p in pics]
         arr = H.host_structs(pics, bufs)
         mutate(arr)
-        lfsim.hostsim_clear_error()
+        lfsim.avb200_clear_error()
         assert lfsim.ff_h263_loop_filter_batch_cuda(C.cast(arr, C.c_void_p), 2, None) == -1, name
-        assert lfsim.hostsim_last_error(), name
+        assert lfsim.avb200_last_error(), name
         assert all(np.array_equal(a, b) for bb, p in zip(bufs, pics) for a, b in zip(bb, p.bufs)), name
 
 
@@ -145,11 +146,11 @@ def test_pictures_sharing_a_frame_are_refused(lfsim):
             arr[2] = arr[0]
         else:
             arr[2].data[1] = arr[1].data[0] + 5 * pics[1].ls
-        lfsim.hostsim_clear_error()
+        lfsim.avb200_clear_error()
         assert lfsim.ff_h263_loop_filter_batch_cuda(C.cast(arr, C.c_void_p), 3, None) == -1
-        assert b"share a frame" in lfsim.hostsim_last_error()
+        assert b"share a frame" in lfsim.avb200_last_error()
         assert all(np.array_equal(a, b) for bb, p in zip(bufs, pics) for a, b in zip(bb, p.bufs))
-    lfsim.hostsim_clear_error()
+    lfsim.avb200_clear_error()
     assert lfsim.ff_h263_loop_filter_batch_cuda(None, 0, None) == 0
     assert lfsim.ff_h263_loop_filter_batch_cuda(None, 2, None) == -1
 
@@ -173,9 +174,9 @@ def test_flush_refuses_a_bad_loop_filter_picture_before_anything_runs(lfsim):
     w = tables.FFMpvPictureWork()
     w.pictures, w.n_pictures, w.rejected = C.cast(C.pointer(mc), C.c_void_p), 1, rej.ctypes.data
     w.loop_filter, w.n_loop_filter = C.cast(larr, C.c_void_p), 1
-    lfsim.hostsim_clear_error()
+    lfsim.avb200_clear_error()
     assert lfsim.ff_mpv_flush_pictures_cuda(C.byref(w), None) == -1
-    assert b"mb_stride" in lfsim.hostsim_last_error()
+    assert b"mb_stride" in lfsim.avb200_last_error()
     assert all(np.array_equal(a, b) for a, b in zip(frame, pic.frame)) and all(np.array_equal(a, b) for a, b in zip(lbufs, lp.bufs))
 
 
@@ -203,7 +204,7 @@ def test_flush_runs_motion_compensation_then_the_loop_filter(lfref, lfsim):
     w = tables.FFMpvPictureWork()
     w.pictures, w.n_pictures, w.rejected = C.cast(C.pointer(mc), C.c_void_p), 1, rej.ctypes.data
     w.loop_filter, w.n_loop_filter = C.cast(C.pointer(lf), C.c_void_p), 1
-    assert lfsim.ff_mpv_flush_pictures_cuda(C.byref(w), None) == 0, lfsim.hostsim_last_error()
+    assert lfsim.ff_mpv_flush_pictures_cuda(C.byref(w), None) == 0, lfsim.avb200_last_error()
     mcd = M.run_ref(M.ref_lib(), pic)
     want = [a.copy() for a in mcd]
     prm = np.array([ls, uvls, 5, 4, tabs.mb_stride], np.int32)

@@ -3,34 +3,17 @@ products) compiled for the host and run block after block over synthetic record 
 size, vectors that leave the picture, `avg` second directions, stacked pictures, unaligned reference planes -- against the compiled
 reference's qpel / chroma tables (tests/h264_util.py::oracle_mc).  TEST INFRASTRUCTURE: the GPU runs the same function per lane
 (tests/test_gpu_h264.py, tests/test_gpu_h264chain.py)."""
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 from libav_b200 import synth
 import h264_util as hu
-
-HERE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-LIB = os.path.join(HERE, "libmc_hostsim.so")
+import hostsim_build
 
 
-@pytest.fixture(scope="session")
+@pytest.fixture
 def mcsim(built):
-    root = os.path.dirname(os.path.dirname(HERE))
-    csrc = os.path.join(root, "libav_b200", "csrc")
-    src = os.path.join(HERE, "mc_block_hostsim.cpp")
-    deps = [src, os.path.join(HERE, "shim", "cuda_runtime.h"), os.path.join(csrc, "h264_mc_block.cuh"), os.path.join(csrc, "common.cuh"),
-            os.path.join(csrc, "h264_residual.cu"), os.path.join(csrc, "h264dsp.cuh"), os.path.join(root, "include", "avdsp_b200.h")]
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in deps):
-        subprocess.run(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-DAVB_HOSTSIM", "-I", HERE, "-I", os.path.join(HERE, "shim"), "-I", csrc,
-                        "-Wno-unknown-pragmas", "-o", LIB, src], check=True)
-    lib = C.CDLL(LIB)
-    lib.hostsim_h264_mc.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.hostsim_h264_residual.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    return lib
+    return hostsim_build.fresh()
 
 
 def run_sim(lib, rec, refs, y, cb, cr, pw, ph, votes):

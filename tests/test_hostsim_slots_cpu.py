@@ -1,43 +1,19 @@
 """CPU: the product's H.264 slot path (libav_b200/csrc/slots.cu + h264dsp.cuh: staging, argument packing, the per-call slot
 kernel, the table hooks) compiled unchanged as host C++ (tests/hostsim/) and driven through the same cases as the GPU tests
-(tests/slot_cases.py), against the oracle.  Not the product and not a fallback: tests/hostsim/libslots_hostsim.so is only ever
-loaded here.  The GPU tests remain the parity tests proper; this keeps the slot code checked while it changes without a GPU."""
+(tests/slot_cases.py), against the oracle.  Not the product and not a fallback: tests/hostsim/libhostsim.so is only ever
+loaded by the CPU suite.  The GPU tests remain the parity tests proper; this keeps the slot code checked while it changes without a GPU."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+import hostsim_build
 import slot_cases
 
-HERE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-LIB = os.path.join(HERE, "libslots_hostsim.so")
 
-
-@pytest.fixture(scope="session")
+@pytest.fixture
 def sim(built):
-    root = os.path.dirname(os.path.dirname(HERE))
-    csrc = os.path.join(root, "libav_b200", "csrc")
-    srcs = [os.path.join(HERE, f) for f in ("slots_hostsim.cpp", "sws_slots_hostsim.cpp", "slots_hbd_hostsim.cpp", "idct10_hostsim.cpp", "h264pred_hbd_hostsim.cpp", "me_cmp_enc_hostsim.cpp", "h264_hbd_hostsim.cpp",
-                                            "swscale_hostsim.cpp")]
-    deps = srcs + [os.path.join(HERE, "shim", "cuda_runtime.h"), os.path.join(HERE, "gen_launches.py")] + \
-        [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cu", ".cuh", ".h"))] + \
-        [os.path.join(root, "include", f) for f in ("avdsp_b200.h", "avdsp_b200_tables.h")]
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in deps):
-        os.makedirs(os.path.join(HERE, "_gen"), exist_ok=True)
-        subprocess.run([sys.executable, os.path.join(HERE, "gen_launches.py"), os.path.join(csrc, "swscale.cu"), os.path.join(HERE, "_gen", "swscale_gen.cu")], check=True)
-        subprocess.run(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-DAVB_HOSTSIM", "-I", os.path.join(HERE, "shim"), "-I", csrc, "-Wno-unknown-pragmas",
-                        "-o", LIB] + srcs, check=True)
-    lib = C.CDLL(LIB)
-    lib.avb200_last_error.restype = C.c_char_p
-    lib.sws_getContext_cuda.restype = C.c_void_p
-    lib.sws_getContext_cuda.argtypes = [C.c_int] * 7 + [C.c_void_p] * 3
-    lib.sws_freeContext_cuda.argtypes = [C.c_void_p]
-    lib.sws_scale_cuda.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-    lib.sws_setColorspaceDetails_cuda.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
-    return lib
+    return hostsim_build.fresh()
 
 
 def last_error_of(lib):

@@ -11,6 +11,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import hostsim_build
 import mpv_mc_cases as M
 
 # (out_format, structure, first_field, b, no_rnd, qpel, bugs, ragged: 1 MPEG-4 size not a multiple of 16, 2 H.263 custom size)
@@ -58,9 +59,9 @@ def mcref(built):
     return lib
 
 
-@pytest.fixture(scope="session")
+@pytest.fixture
 def mcsim(built):
-    return M.sim_lib()
+    return hostsim_build.fresh()
 
 
 @pytest.fixture(scope="session")
@@ -185,9 +186,9 @@ def test_picture_level_refusal(mcsim, field, value):
     s = M.picture_struct(pic, base, base, [a.ctypes.data for a in pic.last], [a.ctypes.data for a in pic.next], recs.ctypes.data, len(recs))
     setattr(s, field, value)
     rej = np.zeros(1, np.uint32)
-    mcsim.hostsim_clear_error()
+    mcsim.avb200_clear_error()
     assert mcsim.ff_mpv_motion_batch_cuda(C.byref(s), 1, rej.ctypes.data, None) == -1
-    assert mcsim.hostsim_last_error()
+    assert mcsim.avb200_last_error()
     assert all(np.array_equal(a, b) for a, b in zip(frame, pic.frame)) and rej[0] == 0
 
 
@@ -200,13 +201,13 @@ def test_h263_field_picture_and_pictures_reading_each_other_are_refused(mcsim):
     b = M.picture_struct(other, frame, frame, [x.ctypes.data for x in pic.last], [x.ctypes.data for x in pic.next], other.recs.ctypes.data, len(other.recs))
     arr = (type(a) * 2)(a, b)
     rej = np.zeros(1, np.uint32)
-    mcsim.hostsim_clear_error()
+    mcsim.avb200_clear_error()
     assert mcsim.ff_mpv_motion_batch_cuda(C.cast(arr, C.c_void_p), 2, rej.ctypes.data, None) == -1
-    assert b"read each other" in mcsim.hostsim_last_error()
+    assert b"read each other" in mcsim.avb200_last_error()
     a.out_format = 2
-    mcsim.hostsim_clear_error()
+    mcsim.avb200_clear_error()
     assert mcsim.ff_mpv_motion_batch_cuda(C.byref(a), 1, rej.ctypes.data, None) == -1
-    assert b"field pictures" in mcsim.hostsim_last_error()
+    assert b"field pictures" in mcsim.avb200_last_error()
 
 
 # ------------------------------------------------------------------------------------------------------------------------ the port
@@ -258,13 +259,13 @@ def test_conflicts_are_found_by_frame_base_without_cur(mcsim):
             s.cur[i] = None
     rej = np.zeros(1, np.uint32)
     arr = (type(sa) * 2)(sa, sb)
-    mcsim.hostsim_clear_error()
+    mcsim.avb200_clear_error()
     assert mcsim.ff_mpv_motion_batch_cuda(C.cast(arr, C.c_void_p), 2, rej.ctypes.data, None) == -1
-    assert b"read each other" in mcsim.hostsim_last_error()
+    assert b"read each other" in mcsim.avb200_last_error()
     own = M.picture_struct(a, base_a, [0, 0, 0], base_a, [x.ctypes.data for x in a.next], a.recs.ctypes.data, len(a.recs))
     for i in range(3):
         own.cur[i] = None
-    mcsim.hostsim_clear_error()
+    mcsim.avb200_clear_error()
     assert mcsim.ff_mpv_motion_batch_cuda(C.byref(own), 1, rej.ctypes.data, None) == -1
-    assert b"being reconstructed" in mcsim.hostsim_last_error()
+    assert b"being reconstructed" in mcsim.avb200_last_error()
     assert all(np.array_equal(x, y) for x, y in zip(fa, a.frame)) and rej[0] == 0

@@ -1,5 +1,5 @@
 """CPU: H.263 overlapped block motion compensation in ff_mpv_motion_batch_cuda.  The product (libav_b200/csrc/mpv_obmc.cuh through
-mpv_mc.cu, compiled for the host by tests/hostsim/h263_hostsim.cpp) and the plain-C port (oracle/port/orc_mpvobmc.c) against the
+mpv_mc.cu, compiled for the host by tests/hostsim/mpv_mc_hostsim.cpp) and the plain-C port (oracle/port/orc_mpvobmc.c) against the
 reference's real ff_mpv_motion with s->obmc set (oracle/_ref/libmpvobmcref.so), whose tables hold each record's raw entries when it runs:
 no_rounding 0 and 1; 16X16 and 8X8 records; intra and missing neighbours on every side; vectors far outside, at and next to every edge,
 custom sizes; right neighbours whose entries disagree with that macroblock's own vectors (the decoder's stale tables); B pictures, where
@@ -9,7 +9,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import h263_cases as H
+import hostsim_build
 import mpv_mc_cases as M
 import mpv_obmc_cases as O
 
@@ -22,9 +22,9 @@ def obref(built):
     return lib
 
 
-@pytest.fixture(scope="module")
+@pytest.fixture
 def obsim(built):
-    return H.sim_lib()
+    return hostsim_build.fresh()
 
 
 @pytest.fixture(scope="module")
@@ -135,7 +135,7 @@ def test_refusals_change_nothing(obsim, field, value):
                     [[a.ctypes.data for a in pic.next]])
     setattr(arr[0], field, value)
     rej = np.zeros(1, np.uint32)
-    obsim.hostsim_clear_error()
+    obsim.avb200_clear_error()
     assert obsim.ff_mpv_motion_batch_cuda(C.cast(arr, C.c_void_p), 1, rej.ctypes.data, None) == -1
-    assert b"OBMC" in obsim.hostsim_last_error()
+    assert b"OBMC" in obsim.avb200_last_error()
     assert all(np.array_equal(a, b) for a, b in zip(frame, pic.frame)) and rej[0] == 0

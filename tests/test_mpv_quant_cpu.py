@@ -14,9 +14,10 @@ import subprocess
 import numpy as np
 import pytest
 
+import hostsim_build
 import mpv_quant_cases as M
 
-ROOT = M.ROOT
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="session")
@@ -32,9 +33,9 @@ def ref(built):
     return r
 
 
-@pytest.fixture(scope="session")
+@pytest.fixture
 def sim(built):
-    return M.sim_lib()
+    return hostsim_build.fresh()
 
 
 def _cases(mats, n=420, seed=0):
@@ -185,7 +186,7 @@ def test_real_trellis_runs(ref, mats):
     fns = [C.c_void_p() for _ in range(3)]
     ref.lib.ref_mpvq_impl.argtypes = [C.POINTER(C.c_void_p)] * 3
     ref.lib.ref_mpvq_impl(*[C.byref(f) for f in fns])
-    lo, hi = _mapping(M.MPVQ_REF)
+    lo, hi = _mapping(ref.lib._name)
     assert all(lo <= f.value < hi for f in fns)
     st = M.make_state(mats, 0, M.FMT_MPEG1, seed=90)
     cur, rf, off, stride = M.planes(300, 17)

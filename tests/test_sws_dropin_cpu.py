@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from test_hostsim_slots_cpu import sim          # noqa: F401  (the fixture that builds / loads tests/hostsim/libslots_hostsim.so)
+from test_hostsim_slots_cpu import sim          # noqa: F401  (the fixture that builds / loads tests/hostsim/libhostsim.so)
 
 
 def test_slots_under_the_reference_scheduler(sim, refo):

@@ -7,17 +7,15 @@ ff_xvid_idct_init_cuda fills; the thread-per-block kernel and the slots compiled
 GPU: ff_xvid_idct_batch_cuda, ff_mpeg_dequant_xvid_idct_batch_cuda and the slots byte for byte against the checker."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from libav_b200 import synth
+import hostsim_build
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 GOLD = os.path.join(HERE, "golden", "fate_idct8x8_xvid.txt")
-XVID_REF = os.path.join(ROOT, "oracle", "_ref", "libxvidref.so")
 NB_ITS = 20000
 FF_IDCT_AUTO, FF_IDCT_INT, FF_IDCT_SIMPLE, FF_IDCT_XVID, FF_IDCT_FAAN = 0, 1, 2, 14, 20
 vp, pd, sz, i32 = C.c_void_p, C.c_ssize_t, C.c_size_t, C.c_int
@@ -57,9 +55,10 @@ def xport(built):
 
 @pytest.fixture(scope="session")
 def xref(built):
-    if not os.path.exists(XVID_REF):
+    from oracle import loader
+    lib = loader.ref_lib("xvid")
+    if lib is None:
         pytest.skip("oracle/_ref not built (no reference tree in this environment)")
-    lib = C.CDLL(XVID_REF)
     lib.ref_xvid_table_fill.restype = i32
     lib.ref_xvid_table_fill.argtypes = [i32, i32, vp, vp, vp]
     return Xvid(lib, "ref_")
@@ -69,7 +68,8 @@ def xref(built):
 def xchk(built):
     """the strongest Xvid checker available: the compiled reference if it travelled, else the port"""
     from oracle import loader
-    return Xvid(C.CDLL(XVID_REF), "ref_") if os.path.exists(XVID_REF) else Xvid(loader.port().lib, "orc_")
+    lib = loader.ref_lib("xvid")
+    return Xvid(lib, "ref_") if lib else Xvid(loader.port().lib, "orc_")
 
 
 # ---------------------------------------------------------------------------------------------------------------------------- cases
@@ -211,38 +211,10 @@ def test_simple_idct_hook_leaves_xvid_alone(built):
     assert not any(_words(t)[3:6])
 
 
-# the host-compiled sources the Xvid library needs: the shim runtime (error channel, scratch pool) of slots_hostsim.cpp, the high-bit-depth
-# table hooks that file's slots.cu refers to, and xvid_idct.cu.  Linked with --no-undefined, so a new dependency of those files is a link
-# error here rather than a library that fails at load time.
-SIM_SOURCES = ("slots_hostsim.cpp", "slots_hbd_hostsim.cpp", "xvid_idct_hostsim.cpp")
-
-
-@pytest.fixture(scope="session")
+@pytest.fixture
 def sim(built):
-    """the product's xvid_idct.cu as host C++ (tests/hostsim/xvid_idct_hostsim.cpp).  Built into its own library, written under a temporary
-    name and renamed into place, so that concurrent test processes never see a half-written file; nothing else under tests/hostsim/ is
-    generated or rewritten."""
-    hs = os.path.join(HERE, "hostsim")
-    csrc = os.path.join(ROOT, "libav_b200", "csrc")
-    lib = os.path.join(hs, "libxvid_hostsim.so")
-    srcs = [os.path.join(hs, f) for f in SIM_SOURCES]
-    deps = srcs + [os.path.join(hs, "shim", "cuda_runtime.h")] + \
-        [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cu", ".cuh", ".h"))] + \
-        [os.path.join(ROOT, "include", f) for f in ("avdsp_b200.h", "avdsp_b200_tables.h")]
-    if not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps):
-        tmp = "%s.%d.tmp" % (lib, os.getpid())
-        try:
-            subprocess.run(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-DAVB_HOSTSIM", "-I", os.path.join(hs, "shim"), "-I", csrc,
-                            "-Wno-unknown-pragmas", "-Wl,--no-undefined", "-o", tmp] + srcs, check=True)
-            os.replace(tmp, lib)
-        finally:
-            if os.path.exists(tmp):
-                os.remove(tmp)
-    s = C.CDLL(lib)
-    s.avb200_last_error.restype = C.c_char_p
-    s.ff_xvid_idct_batch_cuda.argtypes = [i32, vp, vp, vp, pd, sz, i32, i32, vp]
-    s.ff_xvid_idct_init_cuda.argtypes = [vp, i32, i32]
-    return s
+    """the product's xvid_idct.cu as host C++ (tests/hostsim/xvid_idct_hostsim.cpp)"""
+    return hostsim_build.fresh()
 
 
 def test_hostsim_thread_per_block_kernel(sim, xref):
