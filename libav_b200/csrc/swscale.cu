@@ -1265,50 +1265,132 @@ sws_yuyv_yuv422p_kernel(const uint8_t *__restrict__ src, int srcStride, size_t s
 }
 
 // ---------------------------------------------------------------------------------------------------
+// pixel formats
+// ---------------------------------------------------------------------------------------------------
+// AV_PIX_FMT_* values, libavutil/pixfmt.h (the only place the scaler spells them out)
+enum {
+    PIX_YUV420P = 0, PIX_YUYV422 = 1, PIX_RGB24 = 2, PIX_BGR24 = 3, PIX_YUV422P = 4, PIX_YUV444P = 5, PIX_YUV410P = 6, PIX_YUV411P = 7,
+    PIX_GRAY8 = 8, PIX_PAL8 = 11, PIX_YUVJ420P = 12, PIX_YUVJ422P = 13, PIX_YUVJ444P = 14, PIX_UYVY422 = 15, PIX_NV12 = 23, PIX_NV21 = 24,
+    PIX_ARGB = 25, PIX_RGBA = 26, PIX_ABGR = 27, PIX_BGRA = 28, PIX_YUV440P = 31, PIX_YUVJ440P = 32, PIX_YUVA420P = 33,
+    PIX_RGB48BE = 34, PIX_RGB48LE = 35, PIX_RGB565BE = 36, PIX_RGB565LE = 37, PIX_RGB555BE = 38, PIX_RGB555LE = 39,
+    PIX_BGR565BE = 40, PIX_BGR565LE = 41, PIX_BGR555BE = 42, PIX_BGR555LE = 43, PIX_YUV420P16LE = 47, PIX_YUV420P16BE = 48,
+    PIX_YUV422P16LE = 49, PIX_YUV422P16BE = 50, PIX_YUV444P16LE = 51, PIX_YUV444P16BE = 52, PIX_RGB444LE = 54, PIX_RGB444BE = 55,
+    PIX_BGR444LE = 56, PIX_BGR444BE = 57, PIX_BGR48BE = 59, PIX_BGR48LE = 60, PIX_YUV420P9BE = 61, PIX_YUV420P9LE = 62,
+    PIX_YUV420P10BE = 63, PIX_YUV420P10LE = 64, PIX_YUV422P10BE = 65, PIX_YUV422P10LE = 66, PIX_YUV444P9BE = 67, PIX_YUV444P9LE = 68,
+    PIX_YUV444P10BE = 69, PIX_YUV444P10LE = 70, PIX_YUV422P9BE = 71, PIX_YUV422P9LE = 72,
+};
+enum PixFam { FAM_YUV, FAM_NV, FAM_PK422, FAM_RGB24, FAM_RGB32, FAM_RGB16, FAM_RGB48, FAM_GRAY, FAM_PAL8 };
+enum { IN = 1, OUT = 2 };     // the sides a format is taken over on
+
+struct PixFmt {
+    int fmt, side; PixFam fam;
+    int hs, vs;               // chroma sub-sampling, log2 (libavutil/pixdesc.c log2_chroma_w / _h; rgb sources: chosen per context)
+    int bits, be, full;       // sample depth; 16-bit planar samples stored big-endian; full range (yuvj, handle_jpeg, utils.c:855-873)
+    int bpp;                  // bytes per pixel of a packed format
+    int r, g, b, a;           // byte of each channel in a 24 / 32-bit rgb pixel (-1: none)
+    int pk422, rgb16, rgb48, chrStep, slot;     // the SwsDev codes; SwsSlotView::target (-1 planar)
+    int fold;                 // the format the conversion runs as: yuvj -> yuv, yuva420p -> yuv420p (its alpha plane is never read,
+                              // swscale_unscaled.c:1041-1153), 9 / 10 / 16-bit -> its 8-bit layout, gray8 source -> the luma of a 4:4:4 picture
+};
+#define YUV(f, s, hs, vs, bits, be, full, fold) { f, s, FAM_YUV, hs, vs, bits, be, full, 0, -1, -1, -1, -1, 0, 0, 0, 1, -1, fold }
+#define RGB(f, fam, bpp, r, g, b, a, rgb16, rgb48, slot) { f, fam == FAM_RGB16 || fam == FAM_RGB48 ? OUT : IN | OUT, fam, 1, 0, 8, 0, 0, bpp, r, g, b, a, 0, rgb16, rgb48, 1, slot, f }
+static const PixFmt PIXFMTS[] = {
+    YUV(PIX_YUV420P, IN | OUT, 1, 1, 8, 0, 0, PIX_YUV420P),        YUV(PIX_YUVJ420P, IN | OUT, 1, 1, 8, 0, 1, PIX_YUV420P),
+    YUV(PIX_YUV422P, IN | OUT, 1, 0, 8, 0, 0, PIX_YUV422P),        YUV(PIX_YUVJ422P, IN | OUT, 1, 0, 8, 0, 1, PIX_YUV422P),
+    YUV(PIX_YUV444P, IN | OUT, 0, 0, 8, 0, 0, PIX_YUV444P),        YUV(PIX_YUVJ444P, IN | OUT, 0, 0, 8, 0, 1, PIX_YUV444P),
+    YUV(PIX_YUV440P, IN | OUT, 0, 1, 8, 0, 0, PIX_YUV440P),        YUV(PIX_YUVJ440P, IN | OUT, 0, 1, 8, 0, 1, PIX_YUV440P),
+    YUV(PIX_YUV410P, IN | OUT, 2, 2, 8, 0, 0, PIX_YUV410P),        YUV(PIX_YUV411P, IN | OUT, 2, 0, 8, 0, 0, PIX_YUV411P),
+    YUV(PIX_YUVA420P, IN, 1, 1, 8, 0, 0, PIX_YUV420P),
+    YUV(PIX_YUV420P9LE, IN | OUT, 1, 1, 9, 0, 0, PIX_YUV420P),     YUV(PIX_YUV420P9BE, IN | OUT, 1, 1, 9, 1, 0, PIX_YUV420P),
+    YUV(PIX_YUV420P10LE, IN | OUT, 1, 1, 10, 0, 0, PIX_YUV420P),   YUV(PIX_YUV420P10BE, IN | OUT, 1, 1, 10, 1, 0, PIX_YUV420P),
+    YUV(PIX_YUV420P16LE, IN | OUT, 1, 1, 16, 0, 0, PIX_YUV420P),   YUV(PIX_YUV420P16BE, IN | OUT, 1, 1, 16, 1, 0, PIX_YUV420P),
+    YUV(PIX_YUV422P9LE, IN | OUT, 1, 0, 9, 0, 0, PIX_YUV422P),     YUV(PIX_YUV422P9BE, IN | OUT, 1, 0, 9, 1, 0, PIX_YUV422P),
+    YUV(PIX_YUV422P10LE, IN | OUT, 1, 0, 10, 0, 0, PIX_YUV422P),   YUV(PIX_YUV422P10BE, IN | OUT, 1, 0, 10, 1, 0, PIX_YUV422P),
+    YUV(PIX_YUV422P16LE, IN | OUT, 1, 0, 16, 0, 0, PIX_YUV422P),   YUV(PIX_YUV422P16BE, IN | OUT, 1, 0, 16, 1, 0, PIX_YUV422P),
+    YUV(PIX_YUV444P9LE, IN | OUT, 0, 0, 9, 0, 0, PIX_YUV444P),     YUV(PIX_YUV444P9BE, IN | OUT, 0, 0, 9, 1, 0, PIX_YUV444P),
+    YUV(PIX_YUV444P10LE, IN | OUT, 0, 0, 10, 0, 0, PIX_YUV444P),   YUV(PIX_YUV444P10BE, IN | OUT, 0, 0, 10, 1, 0, PIX_YUV444P),
+    YUV(PIX_YUV444P16LE, IN | OUT, 0, 0, 16, 0, 0, PIX_YUV444P),   YUV(PIX_YUV444P16BE, IN | OUT, 0, 0, 16, 1, 0, PIX_YUV444P),
+    // semi-planar: the luma plane and one plane of interleaved chroma (chrStep 2 in the kernels)
+    { PIX_NV12, IN | OUT, FAM_NV, 1, 1, 8, 0, 0, 0, -1, -1, -1, -1, 0, 0, 0, 2, -1, PIX_NV12 },
+    { PIX_NV21, IN | OUT, FAM_NV, 1, 1, 8, 0, 0, 0, -1, -1, -1, -1, 0, 0, 0, 2, -1, PIX_NV21 },
+    { PIX_YUYV422, IN | OUT, FAM_PK422, 1, 0, 8, 0, 0, 2, -1, -1, -1, -1, 1, 0, 0, 1, 2, PIX_YUYV422 },
+    { PIX_UYVY422, IN | OUT, FAM_PK422, 1, 0, 8, 0, 0, 2, -1, -1, -1, -1, 2, 0, 0, 1, 3, PIX_UYVY422 },
+    // gray8: one component (pixdesc); as a destination it becomes a planar stand-in chosen per context
+    { PIX_GRAY8, IN | OUT, FAM_GRAY, 0, 0, 8, 0, 0, 1, -1, -1, -1, -1, 0, 0, 0, 1, -1, PIX_YUV444P },
+    { PIX_PAL8, IN, FAM_PAL8, 0, 0, 8, 0, 0, 1, -1, -1, -1, -1, 0, 0, 0, 1, -1, PIX_PAL8 },
+    RGB(PIX_RGB24, FAM_RGB24, 3, 0, 1, 2, -1, 0, 0, 0),  RGB(PIX_BGR24, FAM_RGB24, 3, 2, 1, 0, -1, 0, 0, 1),
+    RGB(PIX_ARGB, FAM_RGB32, 4, 1, 2, 3, 0, 0, 0, 4),    RGB(PIX_RGBA, FAM_RGB32, 4, 0, 1, 2, 3, 0, 0, 5),
+    RGB(PIX_ABGR, FAM_RGB32, 4, 3, 2, 1, 0, 0, 0, 6),    RGB(PIX_BGRA, FAM_RGB32, 4, 2, 1, 0, 3, 0, 0, 7),
+    // 15 / 16 / 12 bpp: SwsDev::rgb16 1 rgb565 2 bgr565 3 rgb555 4 bgr555 5 rgb444 6 bgr444, + 8 big-endian; 48 bpp: SwsDev::rgb48 1 rgb 2 bgr, + 8 big-endian
+    RGB(PIX_RGB565LE, FAM_RGB16, 2, -1, -1, -1, -1, 1, 0, -1),  RGB(PIX_RGB565BE, FAM_RGB16, 2, -1, -1, -1, -1, 1 | 8, 0, -1),
+    RGB(PIX_BGR565LE, FAM_RGB16, 2, -1, -1, -1, -1, 2, 0, -1),  RGB(PIX_BGR565BE, FAM_RGB16, 2, -1, -1, -1, -1, 2 | 8, 0, -1),
+    RGB(PIX_RGB555LE, FAM_RGB16, 2, -1, -1, -1, -1, 3, 0, -1),  RGB(PIX_RGB555BE, FAM_RGB16, 2, -1, -1, -1, -1, 3 | 8, 0, -1),
+    RGB(PIX_BGR555LE, FAM_RGB16, 2, -1, -1, -1, -1, 4, 0, -1),  RGB(PIX_BGR555BE, FAM_RGB16, 2, -1, -1, -1, -1, 4 | 8, 0, -1),
+    RGB(PIX_RGB444LE, FAM_RGB16, 2, -1, -1, -1, -1, 5, 0, -1),  RGB(PIX_RGB444BE, FAM_RGB16, 2, -1, -1, -1, -1, 5 | 8, 0, -1),
+    RGB(PIX_BGR444LE, FAM_RGB16, 2, -1, -1, -1, -1, 6, 0, -1),  RGB(PIX_BGR444BE, FAM_RGB16, 2, -1, -1, -1, -1, 6 | 8, 0, -1),
+    RGB(PIX_RGB48LE, FAM_RGB48, 6, -1, -1, -1, -1, 0, 1, -1),   RGB(PIX_RGB48BE, FAM_RGB48, 6, -1, -1, -1, -1, 0, 1 | 8, -1),
+    RGB(PIX_BGR48LE, FAM_RGB48, 6, -1, -1, -1, -1, 0, 2, -1),   RGB(PIX_BGR48BE, FAM_RGB48, 6, -1, -1, -1, -1, 0, 2 | 8, -1),
+};
+#undef YUV
+#undef RGB
+
+// the row of a format taken over on `side`, null for anything else
+static const PixFmt *pixfmt(int fmt, int side)
+{
+    for (const PixFmt &f : PIXFMTS) if (f.fmt == fmt) return (f.side & side) ? &f : nullptr;
+    return nullptr;
+}
+static bool is_planar(const PixFmt *f) { return f->fam == FAM_YUV || f->fam == FAM_NV; }
+static bool is_packed_src(const PixFmt *f) { return f->fam == FAM_PK422 || f->fam == FAM_RGB24 || f->fam == FAM_RGB32 || f->fam == FAM_PAL8; }
+
+// ---------------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------------
-enum { FMT_YUV420P = 0, FMT_YUYV422 = 1, FMT_RGB24 = 2, FMT_BGR24 = 3, FMT_YUV422P = 4, FMT_YUV444P = 5, FMT_YUV410P = 6, FMT_YUV411P = 7,
-       FMT_YUVJ420P = 12, FMT_YUVJ422P = 13, FMT_YUVJ444P = 14, FMT_YUVJ440P = 32, FMT_UYVY422 = 15, FMT_ARGB = 25, FMT_RGBA = 26, FMT_ABGR = 27, FMT_BGRA = 28, FMT_NV12 = 23, FMT_NV21 = 24, FMT_YUV440P = 31,
-       FMT_YUV420P16 = 47, FMT_YUV422P16 = 49, FMT_YUV444P16 = 51, FMT_YUV420P9 = 62, FMT_YUV420P10 = 64, FMT_YUV422P10 = 66, FMT_YUV444P9 = 68, FMT_YUV444P10 = 70, FMT_YUV422P9 = 72 };  // libavutil/pixfmt.h (LE)
-
-static bool unscaled0(int sw, int sh, int dw, int dh) { return sw == dw && sh == dh; }
-
-// planar yuv destination: chroma sub-sampling (log2) and sample depth; false for anything else
-static bool planar_dst(int fmt, int *hs, int *vs, int *bits, int *be)
-{
-    *bits = 8; *be = 0;
-    switch (fmt) {               // big-endian twins: 9 / 10-bit LE - 1, 16-bit LE + 1
-    case 61: case 63: case 65: case 67: case 69: case 71: *be = 1; fmt += 1; break;
-    case 48: case 50: case 52: *be = 1; fmt -= 1; break;
-    }
-    switch (fmt) {
-    case FMT_NV12: case FMT_NV21:                          // luma plane + one interleaved chroma plane
-    case FMT_YUV420P: *hs = 1; *vs = 1; return true;
-    case FMT_YUV422P: *hs = 1; *vs = 0; return true;
-    case FMT_YUV444P: *hs = 0; *vs = 0; return true;
-    case FMT_YUV410P: *hs = 2; *vs = 2; return true;
-    case FMT_YUV411P: *hs = 2; *vs = 0; return true;
-    case FMT_YUV440P: *hs = 0; *vs = 1; return true;
-    case FMT_YUV420P9: case FMT_YUV420P10: *hs = 1; *vs = 1; *bits = fmt == FMT_YUV420P9 ? 9 : 10; return true;
-    case FMT_YUV422P9: case FMT_YUV422P10: *hs = 1; *vs = 0; *bits = fmt == FMT_YUV422P9 ? 9 : 10; return true;
-    case FMT_YUV444P9: case FMT_YUV444P10: *hs = 0; *vs = 0; *bits = fmt == FMT_YUV444P9 ? 9 : 10; return true;
-    case FMT_YUV420P16: *hs = 1; *vs = 1; *bits = 16; return true;
-    case FMT_YUV422P16: *hs = 1; *vs = 0; *bits = 16; return true;
-    case FMT_YUV444P16: *hs = 0; *vs = 0; *bits = 16; return true;
-    }
-    return false;
-}
+// The conversion a context runs, chosen once by choose_route() like the reference picks its SwsFunc (utils.c:1043-1054,
+// swscale_unscaled.c:1040-1176).  A packed or semi-planar source reaches the planar routes through a pre-pass (the input readers,
+// input.c, or the nv split), and a 32-bit rgb destination through an expansion of their rgb24 output (run_frames).
+enum Route {
+    R_SCALE,            // swscale(): the tile kernel or the two passes
+    R_FUSED,            // same-size yuv420p -> 24 / 32-bit rgb with identity filters and a 4-tap vertical chroma filter: one kernel
+    R_RGB48,            // 48-bit rgb: sws_rgb48_kernel straight from the source planes
+    R_TABLE,            // the unscaled yuv2rgb table converter (yuv2rgb.c), same-size rgb without SWS_ACCURATE_RND and an even height
+    R_COPY,             // planarCopyWrapper, nv12ToPlanarWrapper
+    R_RGB_COPY,         // rgb24 / bgr24 to itself
+    R_RGB24_SWAP,       // rgb24 <-> bgr24
+    R_BGR24_YV12,       // rgb24toyv12_c
+    R_YUYV_420P,        // yuyv422 / uyvy422 -> yuv420p
+    R_YUYV_422P,        // yuyv422 / uyvy422 -> yuv422p
+    R_RGB_REMAP,        // rgbToRgbWrapper's byte converters: 24 / 32-bit rgb pairs with 32 bits on at least one side
+    R_GRAY_RGB,         // palToRgbWrapper with gray8's pseudo-palette r = g = b = sample
+    R_PAL8_RGB,         // palToRgbWrapper
+    R_422_FROM_422P,    // yuv422p -> yuyv422 / uyvy422
+    R_422_FROM_420P,    // yuv420p -> yuyv422 / uyvy422 (fast-bilinear / point flags only)
+    R_422_COPY,         // yuyv422 / uyvy422 to itself
+    R_NV_INTERLEAVE,    // planarToNv12Wrapper
+};
+static const struct RouteFacts {
+    int plan;           // sws_debug_plan_cuda out[0]
+    bool planar;        // runs on yuv planes: pre-pass for packed / semi-planar sources, expansion for 32-bit rgb destinations
+    bool rowMapped;     // output row y comes from source row y: a slice completes its own rows
+    int chrAlign;       // log2 of the source rows a slice must start on, at least (it also works on whole row pairs)
+    bool tables;        // reads the yuv -> rgb colour tables
+} ROUTES[] = {
+    { 4, true, false, 0, true },  { 3, true, false, 0, true },  { 4, true, false, 0, true },  { 2, true, true, 1, true },
+    { 1, false, true, 0, true },  { 5, false, true, 0, false }, { 5, false, true, 0, false }, { 5, false, true, 1, false },
+    { 5, false, true, 0, false }, { 5, false, true, 0, false }, { 5, false, true, 0, false }, { 5, false, true, 0, false },
+    { 5, false, true, 0, false }, { 6, false, true, 0, true },  { 6, false, true, 1, true },  { 6, false, true, 0, true },
+    { 7, false, true, 0, true },
+};
 
 struct SwsCudaContext {
     SwsGeometry g;
     FilterBank hLum, hChr, vLum, vChr;
     RgbConstants k;
-    int dstFormat;
-    bool copy = false;          // unscaled yuv420p -> yuv420p: the reference installs a plain plane copy
-                                // (utils.c:1043-1054 -> swscale_unscaled.c planarCopyWrapper), whatever the flags
-    bool table_unscaled = false; // same-size rgb without SWS_ACCURATE_RND, even height: the reference's unscaled yuv2rgb SwsFunc
+    const PixFmt *srcFmt, *dstFmt;   // the formats the caller named
+    const PixFmt *S, *D;             // the formats the conversion runs as (PixFmt::fold; a gray8 destination: the planar stand-in, a
+                                     // destination keeps its own depth)
+    Route route;
     bool fast_ok = false;       // the fused interior kernel's host-side preconditions on the filter bank hold
-    bool fused;                 // horizontal identity + vLum identity + 4-tap vChr -> one kernel
     void *d_tables = nullptr;   // all filter banks in one device allocation
     void *d_pair_taps = nullptr; // SwsPairTaps[dstH / 2] for the dp4a fused kernel (fast_ok only)
     void *d_pair_taps_t = nullptr; // SwsPairTapsT[dstH / 2] for the TMA fused kernel (tma_ok only)
@@ -1316,34 +1398,14 @@ struct SwsCudaContext {
     SwsDev dev;
     int16_t *d_lum = nullptr, *d_chrU = nullptr, *d_chrV = nullptr;   // general path line planes
     int lumStridePx = 0, chrStridePx = 0;
-    bool src422 = false;        // the unscaled table converter reads the even chroma line of a 4:2:2 source for both rows (yuv2rgb.c:133-136)
-    int srcNV = 0;              // 0 planar yuv420p, 1 nv12, 2 nv21: semi-planar sources are split into planes first (input.c:475-497)
-    int srcPacked = 0;          // 1 rgb24 / bgr24, 2 yuyv422, 3 uyvy422, 4 argb / rgba / abgr / bgra: the input readers (input.c) write planes first
-    int pkR = 0, pkG = 1, pkB = 2;   //   byte offsets of red, green and blue
-    bool srcGray = false;       // gray8 source: luma only; swscale() never converts chroma lines for it (needs_hcscale, swscale.c:532,768-770) and the vertical stage
-                                // reads what sws_init_context left in the line buffers -- bytes of 64 (utils.c:1273).  Geometry of a format without chroma sub-sampling;
-                                // the entry points hand the kernels the luma plane in place of the two planes the caller does not have (never read)
     uint8_t *d_pal = nullptr;   // pal8 sources through the host-pointer call: the caller's palette (256 x 4 bytes)
-    int srcFormat = 0;          // the source pixel format (after the yuvj / yuva / high-bit-depth twins were folded)
-    int special = 0;            // the reference's unscaled converters for packed sources: 1 rgb copy, 2 rgb24 <-> bgr24, 3 bgr24 -> yuv420p
-                                // (rgb24toyv12_c), 4 yuyv422 -> yuv420p, 5 uyvy422 -> yuv420p, 6 yuyv422 -> yuv422p, 7 uyvy422 -> yuv422p
-    bool planar = false;        // planar yuv destination (else packed rgb)
-    int dst32 = 0;              // argb / rgba / abgr / bgra destination (the pixel format value): rgb24 into d_rgb, then expanded
-    uint8_t *d_rgb = nullptr; size_t rgb_bytes = 0;
-    int dstBits = 8, dstBE = 0;
+    uint8_t *d_rgb = nullptr; size_t rgb_bytes = 0;     // the rgb24 picture a 32-bit destination is expanded from
     int srcRange = 0;           // 1 = full-range (JPEG) source, sws_setColorspaceDetails / a yuvj source format
-    int srcBits = 8, srcBE = 0; // 9 / 10 / 16-bit planar source (16-bit words; hScale16To15_c in the two-pass path)
     int rangeConv = 0;          // yuv destination of the other range: 1 lum / chrRangeFromJpeg_c, 2 lum / chrRangeToJpeg_c on the hscaled lines (two-pass path)
-    int pk422 = 0;              // yuyv422 (1) / uyvy422 (2) destination
-    int rgb16 = 0;              // rgb565 / bgr565 / rgb555 / bgr555 / rgb444 / bgr444 destination (SwsDev::rgb16)
-    int rgb48 = 0;              // rgb48 / bgr48 destination, LE or BE (SwsDev::rgb48)
-    bool gray = false;          // gray8 destination: the luma plane of the planar conversion (swscale.c:618-630 skips the chroma of a gray destination, the
-                                // unscaled copy takes plane 0 only, swscale_unscaled.c:1155); the chroma planes go to scratch nobody reads
+    // gray8 destination: the luma plane of the planar conversion (swscale.c:618-630 skips the chroma of a gray destination, the unscaled
+    // copy takes plane 0 only, swscale_unscaled.c:1155); the chroma planes go to scratch nobody reads
     uint8_t *d_gray[2] = { nullptr, nullptr }; int grayPitch = 0;
     std::vector<uint8_t> h_gray[2];
-    int to422 = 0;              // its unscaled special converters: 1 from yuv422p, 2 from yuv420p (fast-bilinear / point flags only), 3 same-format copy
-    int dstNV = 0;              // 1 nv12, 2 nv21 destination
-    bool nvcopy = false;        // yuv420p -> nv12 / nv21 of the same size: planarToNv12Wrapper
     uint8_t *d_nv = nullptr; size_t nv_bytes = 0;   // the planes the pre-pass of a batch writes (split nv chroma, reader output)
     int2 *d_tile_win = nullptr; size_t tileChrWinOff = 0;
     int tileLumRows = 0, tileChrRows = 0;  // fused-tile general path: shared-memory line capacity; 0 = window too large, two passes
@@ -1369,6 +1431,26 @@ static bool is_identity(const FilterBank &b, int one)
     return true;
 }
 
+// a device copy of a host table; the sticky error is set on failure
+static int upload(void **d, const void *h, size_t bytes)
+{
+    if (cudaMalloc(d, bytes) != cudaSuccess || cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
+        set_error("sws_getContext_cuda", cudaGetLastError()); return -1;
+    }
+    return 0;
+}
+
+// a scratch buffer of at least `need` bytes; an earlier batch on `st` may still use the old one
+static int grow(uint8_t *&buf, size_t &bytes, size_t need, cudaStream_t st, const char *where)
+{
+    if (bytes >= need) return 0;
+    AVB_CUDA(cudaStreamSynchronize(st), where);
+    cudaFree(buf); buf = nullptr; bytes = 0;
+    AVB_CUDA(cudaMalloc(&buf, need), where);
+    bytes = need;
+    return 0;
+}
+
 static int upload_tables(SwsCudaContext *c)
 {
     const FilterBank *banks[4] = { &c->hLum, &c->hChr, &c->vLum, &c->vChr };
@@ -1384,6 +1466,7 @@ static int upload_tables(SwsCudaContext *c)
         AVB_CUDA(cudaMemcpy(base + off[2 * b + 1], banks[b]->pos.data(), banks[b]->pos.size() * 4, cudaMemcpyHostToDevice), "sws:tables");
     }
     SwsDev &d = c->dev;
+    const PixFmt *D = c->D;
     d.srcW = c->g.srcW; d.srcH = c->g.srcH; d.dstW = c->g.dstW; d.dstH = c->g.dstH;
     d.chrSrcW = c->g.chrSrcW; d.chrSrcH = c->g.chrSrcH; d.chrDstW = c->g.chrDstW; d.chrDstH = c->g.chrDstH;
     d.hLumSize = c->hLum.size; d.hChrSize = c->hChr.size; d.vLumSize = c->vLum.size; d.vChrSize = c->vChr.size;
@@ -1392,11 +1475,46 @@ static int upload_tables(SwsCudaContext *c)
     d.vLumF = (const int16_t *)(base + off[4]); d.vLumP = (const int32_t *)(base + off[5]);
     d.vChrF = (const int16_t *)(base + off[6]); d.vChrP = (const int32_t *)(base + off[7]);
     d.k = c->k;
-    d.bgr = c->dstFormat == FMT_BGR24 || (c->rgb48 & 7) == 2;
-    d.full = (c->g.flags & SWS_FULL_CHR_H_INT) != 0 && !c->planar;
-    d.dstBits = c->dstBits; d.dstBE = c->dstBE; d.chrStep = c->dstNV ? 2 : 1; d.pk422 = c->pk422; d.rgb16 = c->rgb16; d.rgb48 = c->rgb48; d.srcGray = c->srcGray;
-    d.srcBits = c->srcBits; d.srcBE = c->srcBE; d.dither = c->srcBits > 8;
+    d.bgr = D->fmt == PIX_BGR24 || (D->rgb48 & 7) == 2;
+    d.full = (c->g.flags & SWS_FULL_CHR_H_INT) != 0 && !is_planar(D);
+    d.dstBits = D->bits; d.dstBE = D->be; d.chrStep = D->chrStep; d.pk422 = D->pk422; d.rgb16 = D->rgb16; d.rgb48 = D->rgb48; d.srcGray = c->srcFmt->fam == FAM_GRAY;
+    d.srcBits = c->srcFmt->bits; d.srcBE = c->srcFmt->be; d.dither = c->srcFmt->bits > 8;
     return 0;
+}
+
+// The route of a context that passed every refusal, its filter banks designed
+static Route choose_route(const SwsCudaContext *c, int flags, bool unscaled, bool usesFilter, bool grayPal, bool rgb2rgb)
+{
+    const PixFmt *S = c->S, *D = c->D;
+    const bool rgb = !is_planar(D), bits8 = c->srcFmt->bits == 8, srcGray = c->srcFmt->fam == FAM_GRAY;
+    if (D->pk422 && unscaled && !usesFilter && !c->rangeConv && bits8) {              // swscale_unscaled.c:1123-1139,1152-1176
+        if (S->fmt == PIX_YUV422P) return R_422_FROM_422P;
+        if (S->fmt == PIX_YUV420P && (flags & (SWS_FAST_BILINEAR | SWS_POINT))) return R_422_FROM_420P;
+        if (S->fmt == D->fmt) return R_422_COPY;
+    }
+    if (D->fam == FAM_NV && S->fmt == PIX_YUV420P && unscaled && !c->rangeConv && bits8) return R_NV_INTERLEAVE;     // swscale_unscaled.c:1040-1044
+    if (unscaled && !usesFilter) {                            // swscale_unscaled.c:1063-1072,1140-1145,1152-1176 (yuv destinations: only with equal ranges, utils.c:1043-1044)
+        if (S->fam == FAM_PAL8 && (D->fam == FAM_RGB24 || D->fam == FAM_RGB32)) return R_PAL8_RGB;       // swscale_unscaled.c:1114-1121
+        if (grayPal) return R_GRAY_RGB;
+        if (rgb2rgb) return R_RGB_REMAP;
+        if (S->fam == FAM_RGB24 && rgb && !D->pk422) return S->fmt == D->fmt ? R_RGB_COPY : R_RGB24_SWAP;
+        // (a gray8 destination is served through a planar stand-in: the reference installs these converters for real yuv420p / yuv422p destinations only)
+        if (!c->rangeConv && c->dstFmt->fam != FAM_GRAY) {
+            if (S->fmt == PIX_BGR24 && D->fmt == PIX_YUV420P && !(flags & SWS_ACCURATE_RND)) return R_BGR24_YV12;
+            if (S->fam == FAM_PK422 && D->fmt == PIX_YUV420P) return R_YUYV_420P;
+            if (S->fam == FAM_PK422 && D->fmt == PIX_YUV422P) return R_YUYV_422P;
+        }
+    }
+    // planarCopyWrapper for planar -> planar of the same size and sub-sampling (swscale_unscaled.c:1152-1176), nv12ToPlanarWrapper for
+    // nv12 / nv21 -> yuv420p (:1046-1049); other nv12 destinations go through swscale()
+    if (D->fam == FAM_YUV && (S->fam == FAM_YUV || (S->fam == FAM_NV && D->fmt == PIX_YUV420P)) && unscaled && ((S->hs == D->hs && S->vs == D->vs) || srcGray) &&
+        !c->rangeConv && !usesFilter && bits8) return R_COPY;
+    // swscale_unscaled.c:1051-1055; the table converter only exists for planar sources (an nv12 frame goes through swscale())
+    if ((S->fmt == PIX_YUV420P || S->fmt == PIX_YUV422P) && rgb && !D->pk422 && unscaled && !(flags & SWS_ACCURATE_RND) && !(c->g.dstH & 1) && !usesFilter && bits8) return R_TABLE;
+    if (D->rgb48) return R_RGB48;
+    if (bits8 && !srcGray && rgb && !D->pk422 && !D->rgb16 && !(flags & SWS_FULL_CHR_H_INT) && !(c->g.flags & SWS_FAST_BILINEAR) && is_identity(c->hLum, 1 << 14) &&
+        is_identity(c->hChr, 1 << 14) && is_identity(c->vLum, 1 << 12) && c->vChr.size == 4) return R_FUSED;
+    return R_SCALE;
 }
 
 struct SwsFilterView { const SwsVec *lumH, *lumV, *chrH, *chrV; };      // libswscale/swscale.h:112-117 (a SwsVector is { double *coeff; int length; })
@@ -1408,137 +1526,82 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
     auto longer = [](const SwsVec *v) { return v && v->length > 1; };
     // usesVFilter / usesHFilter (utils.c:974-981): with either, no unscaled special converter is installed (:1043)
     const bool usesFilter = longer(sf.lumV) || longer(sf.chrV) || longer(df.lumV) || longer(df.chrV) || longer(sf.lumH) || longer(sf.chrH) || longer(df.lumH) || longer(df.chrH);
+    const bool unscaled = srcW == dstW && srcH == dstH;
     const char *err = nullptr;
-    // handle_jpeg() (utils.c:855-873): the full-range planar formats are their limited-range twins with srcRange = 1
-    int srcRange = 0, dstRange = 0;
-    auto handle_jpeg = [](int &fmt) {
-        switch (fmt) {
-        case FMT_YUVJ420P: fmt = FMT_YUV420P; return 1;
-        case FMT_YUVJ422P: fmt = FMT_YUV422P; return 1;
-        case FMT_YUVJ444P: fmt = FMT_YUV444P; return 1;
-        case FMT_YUVJ440P: fmt = FMT_YUV440P; return 1;
-        }
-        return 0;
-    };
-    srcRange = handle_jpeg(srcFormat); dstRange = handle_jpeg(dstFormat);
-    if (srcFormat == 33) {                // AV_PIX_FMT_YUVA420P: the alpha plane is read only when the destination has alpha too (utils.c:1244, yuv2rgb.c:870);
-        // everywhere else the reference treats the format like yuv420p (swscale_unscaled.c:1041-1153): src[3] is never touched
-        if (dstFormat >= FMT_ARGB && dstFormat <= FMT_BGRA) { set_error_msg("sws_getContext_cuda", "yuva420p to a destination with alpha (the alpha plane is scaled too) is not taken over"); return nullptr; }
-        srcFormat = FMT_YUV420P;
+    const PixFmt *srcIn = pixfmt(srcFormat, IN), *dstIn = pixfmt(dstFormat, OUT);
+    const PixFmt *S = srcIn ? pixfmt(srcIn->fold, IN) : nullptr, *D = dstIn && dstIn->full ? pixfmt(dstIn->fold, OUT) : dstIn;
+    const int srcRange = srcIn ? srcIn->full : 0, dstRange = dstIn ? dstIn->full : 0, srcBits = srcIn ? srcIn->bits : 8;
+    const bool srcGray = srcIn && srcIn->fam == FAM_GRAY, gray = dstIn && dstIn->fam == FAM_GRAY;
+    // yuva420p: the alpha plane is read only when the destination has alpha too (utils.c:1244, yuv2rgb.c:870)
+    if (srcIn && srcIn->fmt == PIX_YUVA420P && D && D->fam == FAM_RGB32) {
+        set_error_msg("sws_getContext_cuda", "yuva420p to a destination with alpha (the alpha plane is scaled too) is not taken over"); return nullptr;
     }
-    const bool srcGray = srcFormat == 8;      // AV_PIX_FMT_GRAY8 (pixdesc: one component, log2_chroma_w = log2_chroma_h = 0)
     bool grayPal = false;
     if (srcGray) {
-        const bool d32 = dstFormat >= FMT_ARGB && dstFormat <= FMT_BGRA;
         const char *why = nullptr;
         if (dstRange) why = "gray8 to a full-range yuvj destination (range conversion) is not taken over";
-        else if (dstFormat == FMT_NV12 || dstFormat == FMT_NV21) why = "gray8 to nv12 / nv21 is not taken over (the reference's plane copy fills half of the interleaved chroma row)";
+        else if (D && D->fam == FAM_NV) why = "gray8 to nv12 / nv21 is not taken over (the reference's plane copy fills half of the interleaved chroma row)";
         if (why) { set_error_msg("sws_getContext_cuda", why); return nullptr; }
         // same size to 24 / 32-bit rgb: palToRgbWrapper with the pseudo-palette r = g = b = sample (swscale_unscaled.c:342-384,1114-1121,1257-1259)
-        grayPal = srcW == dstW && srcH == dstH && (dstFormat == FMT_RGB24 || dstFormat == FMT_BGR24 || d32);
-        srcFormat = FMT_YUV444P;
+        grayPal = unscaled && D && (D->fam == FAM_RGB24 || D->fam == FAM_RGB32);
     }
-    // 9 / 10 / 16-bit planar sources (LE values of libavutil/pixfmt.h; big-endian twins: 9 / 10-bit LE - 1, 16-bit LE + 1)
-    int srcBits = 8, srcBE = 0;
-    {
-        int f = srcFormat;
-        if (f == 61 || f == 63 || f == 65 || f == 67 || f == 69 || f == 71) { srcBE = 1; f += 1; }
-        else if (f == 48 || f == 50 || f == 52) { srcBE = 1; f -= 1; }
-        switch (f) {
-        case FMT_YUV420P9: srcBits = 9; srcFormat = FMT_YUV420P; break;   case FMT_YUV420P10: srcBits = 10; srcFormat = FMT_YUV420P; break;
-        case FMT_YUV420P16: srcBits = 16; srcFormat = FMT_YUV420P; break; case FMT_YUV422P9: srcBits = 9; srcFormat = FMT_YUV422P; break;
-        case FMT_YUV422P10: srcBits = 10; srcFormat = FMT_YUV422P; break; case FMT_YUV422P16: srcBits = 16; srcFormat = FMT_YUV422P; break;
-        case FMT_YUV444P9: srcBits = 9; srcFormat = FMT_YUV444P; break;   case FMT_YUV444P10: srcBits = 10; srcFormat = FMT_YUV444P; break;
-        case FMT_YUV444P16: srcBits = 16; srcFormat = FMT_YUV444P; break;
-        default: srcBE = 0; break;
-        }
-    }
-    // gray8 (AV_PIX_FMT_GRAY8 = 8): only luma exists; it is the luma plane of the conversion to a planar yuv picture -- of the source's own
-    // sub-sampling when the source is planar 8-bit yuv, so that the same-size case is the reference's plane copy for every such source
-    // (isPlanarYUV(src) && isGray(dst), swscale_unscaled.c:1155) -- whose chroma planes are written to scratch
-    bool gray = false;
-    if (dstFormat == 8) {
-        gray = true;
-        switch (srcFormat) {
-        case FMT_YUV420P: case FMT_YUV422P: case FMT_YUV444P: case FMT_YUV410P: case FMT_YUV411P: case FMT_YUV440P: dstFormat = srcFormat; break;
-        default: dstFormat = FMT_YUV420P; break;
-        }
-    }
-    int dhs = 1, dvs = 0, dbits = 8, dbe = 0;
-    const bool planar = planar_dst(dstFormat, &dhs, &dvs, &dbits, &dbe);
-    const bool dst32 = dstFormat >= FMT_ARGB && dstFormat <= FMT_BGRA;
-    const int pk422 = dstFormat == FMT_YUYV422 ? 1 : dstFormat == FMT_UYVY422 ? 2 : 0;
-    int rgb16 = 0;                                           // libavutil/pixfmt.h: RGB565BE 36 LE 37, RGB555BE 38 LE 39, BGR565BE 40 LE 41, BGR555BE 42 LE 43, RGB444LE 54 BE 55, BGR444LE 56 BE 57
-    switch (dstFormat) {
-    case 37: rgb16 = 1; break; case 36: rgb16 = 1 | 8; break; case 41: rgb16 = 2; break; case 40: rgb16 = 2 | 8; break;
-    case 39: rgb16 = 3; break; case 38: rgb16 = 3 | 8; break; case 43: rgb16 = 4; break; case 42: rgb16 = 4 | 8; break;
-    case 54: rgb16 = 5; break; case 55: rgb16 = 5 | 8; break; case 56: rgb16 = 6; break; case 57: rgb16 = 6 | 8; break;
-    }
-    const int rgb48 = dstFormat == 35 ? 1 : dstFormat == 34 ? 1 | 8 : dstFormat == 60 ? 2 : dstFormat == 59 ? 2 | 8 : 0;      // RGB48BE 34 LE 35, BGR48BE 59 LE 60
-    if (pk422 || rgb16 || rgb48) flags &= ~SWS_FULL_CHR_H_INT;        // only 24 / 32-bit packed RGB knows the flag (utils.c:998-1014)
-    if (!planar && dstFormat != FMT_RGB24 && dstFormat != FMT_BGR24 && !dst32 && !pk422 && !rgb16 && !rgb48) {
+    // gray8 destination: the luma plane of the conversion to a planar yuv picture -- of the source's own sub-sampling when the source is
+    // planar 8-bit yuv, so that the same-size case is the reference's plane copy for every such source (isPlanarYUV(src) && isGray(dst),
+    // swscale_unscaled.c:1155) -- whose chroma planes are written to scratch
+    if (gray) D = pixfmt(S && S->fam == FAM_YUV ? S->fmt : PIX_YUV420P, OUT);
+    if (!D) {
         set_error_msg("sws_getContext_cuda", "destinations taken over: gray8, rgb24, bgr24, argb, rgba, abgr, bgra, rgb48 / bgr48 (LE and BE), rgb565 / bgr565 / rgb555 / bgr555 / rgb444 / bgr444 (LE and BE), yuyv422, uyvy422, nv12, nv21, planar yuv 420p 422p 444p 410p 411p 440p, 9 / 10 / 16-bit 420p 422p 444p (LE and BE)");
         return nullptr;
     }
+    const bool planar = is_planar(D), rgb = !planar;
+    if (D->pk422 || D->rgb16 || D->rgb48) flags &= ~SWS_FULL_CHR_H_INT;        // only 24 / 32-bit packed RGB knows the flag (utils.c:998-1014)
     if (flags & 0x30000) {                                    // SWS_SRC_V_CHR_DROP_MASK (utils.c:1016-1019, swscale.c:383-384)
         set_error_msg("sws_getContext_cuda", "SWS_SRC_V_CHR_DROP (skipping source chroma lines) is not taken over"); return nullptr;
     }
-    int hs = 1, vs = 1;                                       // source chroma sub-sampling, libavutil/pixdesc.c log2_chroma_w / _h
-    switch (srcFormat) {
-    case FMT_YUV420P: case FMT_NV12: case FMT_NV21: break;
-    case FMT_YUV422P: vs = 0; break;
-    case FMT_YUV444P: hs = 0; vs = 0; break;
-    case FMT_YUV410P: hs = 2; vs = 2; break;
-    case FMT_YUV411P: hs = 2; vs = 0; break;
-    case FMT_YUV440P: hs = 0; break;
-    case FMT_YUYV422: case FMT_UYVY422: vs = 0; break;
-    case 11: hs = 0; vs = 0; break;                            // AV_PIX_FMT_PAL8 (pixdesc: one component, no chroma sub-sampling; its readers give chroma per pixel)
-    case FMT_RGB24: case FMT_BGR24: case FMT_ARGB: case FMT_RGBA: case FMT_ABGR: case FMT_BGRA: {   // utils.c:1021-1034: every other pixel for chroma unless told / forced otherwise
-        const int chrDstHSub = planar ? dhs : (flags & SWS_FULL_CHR_H_INT) ? 0 : 1;
+    if (!S) {
+        set_error_msg("sws_getContext_cuda", "sources taken over: planar 8-bit yuv (420p 422p 444p 410p 411p 440p, yuvj, yuva420p), gray8, 9 / 10 / 16-bit planar yuv, nv12, nv21, yuyv422, uyvy422, rgb24, bgr24, argb, rgba, abgr, bgra");
+        return nullptr;
+    }
+    const bool srcRgb = S->fam == FAM_RGB24, src32 = S->fam == FAM_RGB32, srcYuy = S->fam == FAM_PK422, srcPal = S->fam == FAM_PAL8, srcNV = S->fam == FAM_NV;
+    const bool dst32 = D->fam == FAM_RGB32, dstNV = D->fam == FAM_NV;
+    int hs = S->hs, vs = S->vs;
+    if (srcRgb || src32) {      // utils.c:1021-1034: every other pixel for chroma unless told / forced otherwise
+        const int chrDstHSub = planar ? D->hs : (flags & SWS_FULL_CHR_H_INT) ? 0 : 1;
         hs = (!(flags & SWS_FULL_CHR_H_INP) && ((dstW >> chrDstHSub) <= (srcW >> 1) || (flags & SWS_FAST_BILINEAR))) ? 1 : 0;
-        vs = 0;
-        break;
     }
-    default: set_error_msg("sws_getContext_cuda", "sources taken over: planar 8-bit yuv (420p 422p 444p 410p 411p 440p, yuvj, yuva420p), gray8, 9 / 10 / 16-bit planar yuv, nv12, nv21, yuyv422, uyvy422, rgb24, bgr24, argb, rgba, abgr, bgra"); return nullptr;
-    }
-    if ((srcFormat == FMT_NV12 || srcFormat == FMT_NV21) && (dstFormat == FMT_NV12 || dstFormat == FMT_NV21) && srcW == dstW && srcH == dstH) {
+    if (srcNV && dstNV && unscaled) {
         set_error_msg("sws_getContext_cuda", "nv12 / nv21 -> nv12 / nv21 of the same size (the reference's plane copy skips the chroma plane there) is not taken over"); return nullptr;
     }
-    const bool src32 = srcFormat >= FMT_ARGB && srcFormat <= FMT_BGRA;
     // same size, packed rgb on both sides, 32 bits on at least one: rgbToRgbWrapper's byte converters (swscale_unscaled.c:590-705), a channel remap
-    const bool rgb2rgb = unscaled0(srcW, srcH, dstW, dstH) && !usesFilter && (srcFormat == FMT_RGB24 || srcFormat == FMT_BGR24 || src32) &&
-                         (dstFormat == FMT_RGB24 || dstFormat == FMT_BGR24 || dst32) && (src32 || dst32);
-    if (src32 && !rgb2rgb && (dst32 || (unscaled0(srcW, srcH, dstW, dstH) && !planar && !pk422))) {
+    const bool rgb2rgb = unscaled && !usesFilter && (srcRgb || src32) && (D->fam == FAM_RGB24 || dst32) && (src32 || dst32);
+    if (src32 && !rgb2rgb && (dst32 || (unscaled && !planar && !D->pk422))) {
         // 32 -> 32 bit at another size: the reference scales the alpha plane too; same size -> 16 / 48-bit rgb: other converter families
         set_error_msg("sws_getContext_cuda", "32-bit rgb source: planar yuv destinations, scaled rgb24 / bgr24 and same-size 24 / 32-bit rgb are taken over"); return nullptr;
     }
-    const bool srcRgb = srcFormat == FMT_RGB24 || srcFormat == FMT_BGR24, srcYuy = srcFormat == FMT_YUYV422 || srcFormat == FMT_UYVY422, srcPal = srcFormat == 11;
-    const bool unscaled = srcW == dstW && srcH == dstH;
-    if (dstFormat == FMT_ABGR && (flags & SWS_FULL_CHR_H_INT) && !grayPal && !rgb2rgb && !(srcPal && unscaled && !usesFilter)) {      // (the unscaled converters never reach that output function)  // output.c:1231-1237 advances the pointer twice per abgr pixel and runs off the row
+    if (D->fmt == PIX_ABGR && (flags & SWS_FULL_CHR_H_INT) && !grayPal && !rgb2rgb && !(srcPal && unscaled && !usesFilter)) {      // (the unscaled converters never reach that output function)  // output.c:1231-1237 advances the pointer twice per abgr pixel and runs off the row
         set_error_msg("sws_getContext_cuda", "abgr with SWS_FULL_CHR_H_INT: the reference's output function overruns the destination; there is no result to match");
         return nullptr;
     }
-    if (srcRgb && unscaled && (dstFormat == FMT_ARGB || dstFormat == FMT_ABGR)) {
+    if (srcRgb && unscaled && (D->fmt == PIX_ARGB || D->fmt == PIX_ABGR)) {
         // rgbToRgbWrapper moves the 4-byte writer one byte into the row for these two (ALT32_CORR, swscale_unscaled.c:691-692): the first alpha byte is
         // never written and the last write lands past the row
         set_error_msg("sws_getContext_cuda", "rgb24 / bgr24 -> argb / abgr of the same size: the reference's converter writes past the row; there is no result to match");
         return nullptr;
     }
-    if (srcFormat == FMT_BGR24 && dstFormat == FMT_YUV420P && !gray && unscaled && !(flags & SWS_ACCURATE_RND) && (srcH & 1) && srcRange == dstRange) {
+    if (S->fmt == PIX_BGR24 && D->fmt == PIX_YUV420P && !gray && unscaled && !(flags & SWS_ACCURATE_RND) && (srcH & 1) && srcRange == dstRange) {
         set_error_msg("sws_getContext_cuda", "bgr24 -> yuv420p of the same size without SWS_ACCURATE_RND is the reference's rgb24toyv12, which needs an even height");
         return nullptr;
     }
-    if (srcFormat == FMT_YUV410P && dstFormat == FMT_YUV420P && srcW == dstW && srcH == dstH && !(flags & SWS_BITEXACT) && srcRange == dstRange) {
+    if (S->fmt == PIX_YUV410P && D->fmt == PIX_YUV420P && unscaled && !(flags & SWS_BITEXACT) && srcRange == dstRange) {
         set_error_msg("sws_getContext_cuda", "yuv410p -> yuv420p of the same size without SWS_BITEXACT is the reference's yvu9ToYv12Wrapper: not taken over");
         return nullptr;
     }
-    const bool rgb = !planar;
-    if (rgb16) {
+    if (D->rgb16) {
         // the 15 / 16 / 12-bpp destinations exist where swscale()'s packed output stage runs (yuv2rgb16_X / _2 / _1 ..., output.c:1321-1326);
         // the reference's other routes to them are separate converter families that are not taken over
         const char *why = nullptr;
         if (srcRgb || src32 || srcYuy || srcPal) why = "15 / 16 / 12-bpp rgb destinations are taken over for planar / semi-planar yuv sources only";
-        else if ((srcFormat == FMT_YUV420P || srcFormat == FMT_YUV422P) && unscaled && !(flags & SWS_ACCURATE_RND) && !(dstH & 1) && !usesFilter && srcBits == 8)
+        else if ((S->fmt == PIX_YUV420P || S->fmt == PIX_YUV422P) && unscaled && !(flags & SWS_ACCURATE_RND) && !(dstH & 1) && !usesFilter && srcBits == 8)
             why = "same-size yuv -> 15 / 16 / 12-bpp rgb without SWS_ACCURATE_RND is the reference's ordered-dither table converter (yuv2rgb.c:377-573): not taken over";
         else if (usesFilter) why = "SwsFilter vectors with a 15 / 16 / 12-bpp destination are not taken over";
         if (why) { set_error_msg("sws_getContext_cuda", why); return nullptr; }
@@ -1546,14 +1609,14 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
     if (srcGray) {
         const char *why = nullptr;
         if (usesFilter) why = "SwsFilter vectors with a gray8 source are not taken over";
-        else if (planar && dbits == 16) why = "gray8 to a 16-bit planar destination is not taken over";
-        else if (planar && dbits != 8 && srcW == dstW && srcH == dstH) why = "gray8 to a 9 / 10-bit planar destination of the same size (planarCopyWrapper's fill_plane9or10) is not taken over";
+        else if (planar && D->bits == 16) why = "gray8 to a 16-bit planar destination is not taken over";
+        else if (planar && D->bits != 8 && unscaled) why = "gray8 to a 9 / 10-bit planar destination of the same size (planarCopyWrapper's fill_plane9or10) is not taken over";
         if (why) { set_error_msg("sws_getContext_cuda", why); return nullptr; }
     }
-    if (rgb48) {
+    if (D->rgb48) {
         // 48-bit destinations: the packed output stage on hScale8To19_c lines, and the unscaled table converter; planar 8-bit yuv sources
         const char *why = nullptr;
-        if (srcRgb || src32 || srcYuy || srcPal || srcFormat == FMT_NV12 || srcFormat == FMT_NV21) why = "48-bit rgb destinations are taken over for planar 8-bit yuv sources only";
+        if (srcRgb || src32 || srcYuy || srcPal || srcNV) why = "48-bit rgb destinations are taken over for planar 8-bit yuv sources only";
         else if (srcBits > 8) why = "9 / 10 / 16-bit source to a 48-bit rgb destination (hScale16To19_c lines) is not taken over";
         else if (usesFilter) why = "SwsFilter vectors with a 48-bit rgb destination are not taken over";
         if (why) { set_error_msg("sws_getContext_cuda", why); return nullptr; }
@@ -1563,14 +1626,14 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
         auto asym = [](const SwsVec *v) { if (!v) return false; for (int i = 0; i < v->length / 2; i++) if (v->coeff[i] != v->coeff[v->length - 1 - i]) return true; return false; };
         if (asym(sf.lumV) || asym(sf.chrV)) { set_error_msg("sws_getContext_cuda", "asymmetric vertical SwsFilter vectors are not taken over"); return nullptr; }
     }
-    if (usesFilter && (srcRgb || srcYuy || src32 || srcPal || srcFormat == FMT_NV12 || srcFormat == FMT_NV21 || pk422 || dstFormat == FMT_NV12 || dstFormat == FMT_NV21 || dbits != 8)) {
+    if (usesFilter && (srcRgb || srcYuy || src32 || srcPal || srcNV || D->pk422 || dstNV || D->bits != 8)) {
         set_error_msg("sws_getContext_cuda", "SwsFilter vectors are taken over for planar 8-bit yuv sources to packed rgb / planar 8-bit yuv destinations only");
         return nullptr;
     }
     // swscale.c:748-765: a yuv destination of the other range gets lum / chrRangeFromJpeg_c (1) or ...ToJpeg_c (2) between the two passes,
     // and none of the unscaled special converters (utils.c:1043-1044)
-    const int rangeConv = (srcRange != dstRange && (planar || pk422)) ? (srcRange ? 1 : 2) : 0;
-    if (rangeConv && dbits == 16) {       // (the *Range*16_c variants work on the 19-bit lines that only exist in the tile kernel)
+    const int rangeConv = (srcRange != dstRange && (planar || D->pk422)) ? (srcRange ? 1 : 2) : 0;
+    if (rangeConv && D->bits == 16) {       // (the *Range*16_c variants work on the 19-bit lines that only exist in the tile kernel)
         set_error_msg("sws_getContext_cuda", "range conversion (full-range yuvj <-> limited-range yuv) to a 16-bit destination is not taken over");
         return nullptr;
     }
@@ -1578,44 +1641,18 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
         const char *why = nullptr;
         if (usesFilter) why = "SwsFilter vectors with a 9 / 10 / 16-bit source are not taken over";
         else if (rangeConv) why = "range conversion from a 9 / 10 / 16-bit source is not taken over";
-        else if (planar && dbits == 16) why = "9 / 10 / 16-bit source to a 16-bit destination (hScale16To19_c lines) is not taken over";
+        else if (planar && D->bits == 16) why = "9 / 10 / 16-bit source to a 16-bit destination (hScale16To19_c lines) is not taken over";
         // same size and sub-sampling, planar destination: planarCopyWrapper with its own depth conversions (swscale_unscaled.c:793-1020)
-        else if (planar && dstFormat != FMT_NV12 && dstFormat != FMT_NV21 && srcW == dstW && srcH == dstH && hs == dhs && vs == dvs)
+        else if (planar && !dstNV && unscaled && hs == D->hs && vs == D->vs)
             why = "9 / 10 / 16-bit source to a planar destination of the same size and sub-sampling is the reference's planarCopyWrapper: not taken over";
         if (why) { set_error_msg("sws_getContext_cuda", why); return nullptr; }
     }
     if (!rgb) flags &= ~SWS_FULL_CHR_H_INT;                 // only packed RGB knows the flag (utils.c:998-1014)
     SwsCudaContext *c = new (std::nothrow) SwsCudaContext();
     if (!c) return nullptr;
-    c->pk422 = pk422; c->rgb16 = rgb16; c->rgb48 = rgb48; c->srcGray = srcGray; c->gray = gray; c->srcBits = srcBits; c->srcBE = srcBE;
-    if (pk422 && srcW == dstW && srcH == dstH && !usesFilter && !rangeConv && srcBits == 8) {               // swscale_unscaled.c:1123-1139,1152-1176
-        if (srcFormat == FMT_YUV422P) c->to422 = 1;
-        else if (srcFormat == FMT_YUV420P && (flags & (SWS_FAST_BILINEAR | SWS_POINT))) c->to422 = 2;
-        else if (srcFormat == dstFormat) c->to422 = 3;
-    }
-    c->dstNV = dstFormat == FMT_NV12 ? 1 : dstFormat == FMT_NV21 ? 2 : 0;
-    c->dstFormat = dstFormat; c->dst32 = dst32 ? dstFormat : 0; c->planar = planar; c->dstBits = dbits; c->dstBE = dbe;
-    c->srcNV = srcFormat == FMT_NV12 ? 1 : srcFormat == FMT_NV21 ? 2 : 0;
+    c->srcFmt = srcIn; c->dstFmt = dstIn; c->S = S; c->D = D; c->rangeConv = rangeConv;
     double prm[2] = { param ? param[0] : SWS_PARAM_DEFAULT, param ? param[1] : SWS_PARAM_DEFAULT };
-    c->src422 = srcFormat == FMT_YUV422P && srcBits == 8;
-    c->srcPacked = srcRgb ? 1 : srcFormat == FMT_YUYV422 ? 2 : srcFormat == FMT_UYVY422 ? 3 : src32 ? 4 : srcPal ? 5 : 0;
-    c->pkR = srcFormat == FMT_BGR24 ? 2 : 0; c->pkB = 2 - c->pkR; c->srcFormat = srcFormat;
-    if (src32) {
-        static const int rgbpos[4][3] = { { 1, 2, 3 }, { 0, 1, 2 }, { 3, 2, 1 }, { 2, 1, 0 } };       // argb, rgba, abgr, bgra
-        c->pkR = rgbpos[srcFormat - FMT_ARGB][0]; c->pkG = rgbpos[srcFormat - FMT_ARGB][1]; c->pkB = rgbpos[srcFormat - FMT_ARGB][2];
-    }
-    if (unscaled && !usesFilter) {                            // swscale_unscaled.c:1063-1072,1140-1145,1152-1176 (yuv destinations: only with equal ranges, utils.c:1043-1044)
-        if (srcPal && (dstFormat == FMT_RGB24 || dstFormat == FMT_BGR24 || dst32)) c->special = 10;      // palToRgbWrapper (swscale_unscaled.c:1114-1121)
-        else if (grayPal) c->special = 9;
-        else if (rgb2rgb) c->special = 8;
-        else if (srcRgb && rgb && !pk422) c->special = srcFormat == dstFormat ? 1 : 2;
-        else if (rangeConv) c->special = 0;
-        // (a gray8 destination is served through a planar stand-in: the reference installs these converters for real yuv420p / yuv422p destinations only)
-        else if (srcFormat == FMT_BGR24 && dstFormat == FMT_YUV420P && !gray && !(flags & SWS_ACCURATE_RND)) c->special = 3;
-        else if (srcYuy && dstFormat == FMT_YUV420P && !gray) c->special = srcFormat == FMT_YUYV422 ? 4 : 5;
-        else if (srcYuy && dstFormat == FMT_YUV422P && !gray) c->special = srcFormat == FMT_YUYV422 ? 6 : 7;
-    }
-    if (derive_geometry(c->g, srcW, srcH, dstW, dstH, rgb, flags, &err, hs, vs, dhs, dvs)) goto fail;
+    if (derive_geometry(c->g, srcW, srcH, dstW, dstH, rgb, flags, &err, hs, vs, D->hs, D->vs)) goto fail;
     {
         const int fl = c->g.flags;
         const int lumFlags = (fl & SWS_BICUBLIN) ? (fl | SWS_BICUBIC) : fl;
@@ -1630,11 +1667,8 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
         rgb_constants(c->k, itu601, srcRange, 0, 1 << 16, 1 << 16);      // sws_getContext defaults, utils.c:1366-1368
         c->srcRange = srcRange;
     }
-    // swscale_unscaled.c:1051-1055; the table converter only exists for planar sources (an nv12 frame goes through swscale())
-    c->table_unscaled = (srcFormat == FMT_YUV420P || srcFormat == FMT_YUV422P) && rgb && !pk422 && srcW == dstW && srcH == dstH && !(flags & SWS_ACCURATE_RND) && !(dstH & 1) && !usesFilter && srcBits == 8;
-    c->fused = srcBits == 8 && !srcGray && !c->table_unscaled && rgb && !pk422 && !rgb16 && !rgb48 && !(flags & SWS_FULL_CHR_H_INT) && !(c->g.flags & SWS_FAST_BILINEAR) && is_identity(c->hLum, 1 << 14) && is_identity(c->hChr, 1 << 14) && is_identity(c->vLum, 1 << 12) &&
-               c->vChr.size == 4;
-    if (c->fused && !(dstW & 15) && !(dstH & 1)) {
+    c->route = choose_route(c, flags, unscaled, usesFilter, grayPal, rgb2rgb);
+    if (c->route == R_FUSED && !(dstW & 15) && !(dstH & 1)) {
         bool ok = true;
         for (int y = 0; y < dstH && ok; y += 2) {
             const int f0 = c->vChr.pos[y] > -3 ? c->vChr.pos[y] : -3, f1 = c->vChr.pos[y + 1] > -3 ? c->vChr.pos[y + 1] : -3;
@@ -1647,15 +1681,10 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
         }
         c->fast_ok = ok;
     }
-    // planarCopyWrapper for planar -> planar of the same size and sub-sampling (swscale_unscaled.c:1152-1176), nv12ToPlanarWrapper for
-    // nv12 / nv21 -> yuv420p (:1046-1049); other nv12 destinations go through swscale()
-    c->copy = planar && !c->dstNV && !c->srcPacked && srcW == dstW && srcH == dstH && ((hs == dhs && vs == dvs) || srcGray) && (!c->srcNV || dstFormat == FMT_YUV420P) && !rangeConv && !usesFilter && srcBits == 8;
-    c->rangeConv = rangeConv;
-    c->nvcopy = c->dstNV && srcFormat == FMT_YUV420P && srcW == dstW && srcH == dstH && !rangeConv && srcBits == 8;           // swscale_unscaled.c:1040-1044
     if (!device_side) return c;
     if (upload_tables(c)) { destroy(c); return nullptr; }
     if (srcPal && cudaMalloc(&c->d_pal, 1024) != cudaSuccess) { set_error("sws_getContext_cuda", cudaGetLastError()); destroy(c); return nullptr; }
-    if (c->gray) {
+    if (gray) {
         c->grayPitch = (c->g.chrDstW + 63) & ~31;
         for (int k = 0; k < 2; k++)
             if (cudaMalloc(&c->d_gray[k], (size_t)c->grayPitch * (c->g.chrDstH + 2)) != cudaSuccess) { set_error("sws_getContext_cuda", cudaGetLastError()); destroy(c); return nullptr; }
@@ -1676,12 +1705,7 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
             t.tap4 = k1[4]; t.first = f0;
             pt[rp] = t;
         }
-        if (c->fast_ok) {
-            if (cudaMalloc(&c->d_pair_taps, pt.size() * sizeof(SwsPairTaps)) != cudaSuccess ||
-                cudaMemcpy(c->d_pair_taps, pt.data(), pt.size() * sizeof(SwsPairTaps), cudaMemcpyHostToDevice) != cudaSuccess) {
-                set_error("sws_getContext_cuda", cudaGetLastError()); destroy(c); return nullptr;
-            }
-        }
+        if (c->fast_ok && upload(&c->d_pair_taps, pt.data(), pt.size() * sizeof(SwsPairTaps))) { destroy(c); return nullptr; }
     }
     if (c->fast_ok) {            // the TMA kernel's table: per pair the int16 tap pairs of both rows, per four-pair tile its chroma line window
         const int pairs = dstH / 2, chrH = c->g.chrSrcH;
@@ -1710,14 +1734,11 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
             for (int rp = t0; rp < t1; rp++) { pt[rp].base = lo; pt[rp].interior = interior; }
         }
         if (ok && pairs > 0) {
-            if (cudaMalloc(&c->d_pair_taps_t, pt.size() * sizeof(SwsPairTapsT)) != cudaSuccess ||
-                cudaMemcpy(c->d_pair_taps_t, pt.data(), pt.size() * sizeof(SwsPairTapsT), cudaMemcpyHostToDevice) != cudaSuccess) {
-                set_error("sws_getContext_cuda", cudaGetLastError()); destroy(c); return nullptr;
-            }
+            if (upload(&c->d_pair_taps_t, pt.data(), pt.size() * sizeof(SwsPairTapsT))) { destroy(c); return nullptr; }
             c->tma_ok = true;
         }
     }
-    if (!c->fused && !c->copy && !c->table_unscaled && !c->to422 && !rgb48) {          // (rgb48: sws_rgb48_kernel works from the source planes, no line planes)
+    if (c->route == R_SCALE) {
         int lr = 0, cr = 0, lo, hi;
         std::vector<int2> win;
         for (int y0 = 0; y0 < dstH; y0 += GT_H) {
@@ -1732,15 +1753,12 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
         }
         const bool fullc = rgb && (flags & SWS_FULL_CHR_H_INT);
         const size_t need = rgb ? ((size_t)lr * GT_LW + (size_t)cr * (fullc ? 2 * GT_LW : GT_W)) * 4 : (size_t)std::max(lr, cr) * GT_LW * 4;
-        if (need <= 96 * 1024 && !pk422 && !rgb16 && !rangeConv && srcBits == 8 && !srcGray) {          // (the packed 4:2:2 / 16-bpp output stages and the range conversion only exist in the two-pass path so far)
+        if (need <= 96 * 1024 && !D->pk422 && !D->rgb16 && !rangeConv && srcBits == 8 && !srcGray) {          // (the packed 4:2:2 / 16-bpp output stages and the range conversion only exist in the two-pass path so far)
             c->tileLumRows = lr; c->tileChrRows = cr;
-            if (cudaMalloc(&c->d_tile_win, win.size() * sizeof(int2)) != cudaSuccess ||
-                cudaMemcpy(c->d_tile_win, win.data(), win.size() * sizeof(int2), cudaMemcpyHostToDevice) != cudaSuccess) {
-                set_error("sws_getContext_cuda", cudaGetLastError()); destroy(c); return nullptr;
-            }
+            if (upload((void **)&c->d_tile_win, win.data(), win.size() * sizeof(int2))) { destroy(c); return nullptr; }
             c->tileChrWinOff = nLumWin;
         }
-        if (dbits == 16 && !c->tileLumRows) {      // the two-pass fallback keeps 15-bit lines in int16 planes
+        if (D->bits == 16 && !c->tileLumRows) {      // the two-pass fallback keeps 15-bit lines in int16 planes
             set_error_msg("sws_getContext_cuda", "16-bit destination: the vertical filter window does not fit in shared memory (19-bit lines exist only there)");
             destroy(c); return nullptr;
         }
@@ -1760,200 +1778,70 @@ fail:
     return nullptr;
 }
 
-static int run_planar(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
-                      uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st);
-
-// semi-planar sources: split the interleaved chroma plane, then everything is the planar path.  Same-size planar output is
-// Packed sources (rgb24 / bgr24 / yuyv422 / uyvy422): the reference's unscaled special converters where it installs them, else the
-// input readers into planes (one pre-pass, + srcW * srcH * (1 + 2 / 2^hs) bytes written and read again) and the planar kernels.
-static int run_packed(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
-                      uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st)
+// ---------------------------------------------------------------------------------------------------
+// what a context reads and writes
+// ---------------------------------------------------------------------------------------------------
+// The planes of a picture as the caller lays them out: how many, the bytes of a row's pixels, the rows
+struct PlaneGeom { int n; size_t row[3]; int rows[3]; };
+static PlaneGeom src_planes(const SwsCudaContext *c)
 {
-    if (nframes <= 0) return 0;
-    const SwsDev &p = c->dev;
-    const int w = p.srcW, h = p.srcH;
-    if (c->special == 8) {
-        // byte of r, g, b, a in rgb24, bgr24, argb, rgba, abgr, bgra
-        static const int chan[6][4] = { { 0, 1, 2, -1 }, { 2, 1, 0, -1 }, { 1, 2, 3, 0 }, { 0, 1, 2, 3 }, { 3, 2, 1, 0 }, { 2, 1, 0, 3 } };
-        const int sf = c->srcPacked == 4 ? 2 + c->srcFormat - FMT_ARGB : c->srcFormat == FMT_BGR24 ? 1 : 0, df = c->dst32 ? 2 + c->dst32 - FMT_ARGB : c->dstFormat == FMT_BGR24 ? 1 : 0;
-        const int sbpp = c->srcPacked == 4 ? 4 : 3, dbpp = c->dst32 ? 4 : 3;
-        unsigned map = 0;
-        for (int ch = 0; ch < 4; ch++) if (chan[df][ch] >= 0) map |= (unsigned)(chan[sf][ch] >= 0 ? chan[sf][ch] : 15) << (4 * chan[df][ch]);
-        sws_rgb_map_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dstStride[0], dstFrame[0], w, h, sbpp, dbpp, map);
-        return check_launch("sws_scale:rgb2rgb");
-    }
-    if (c->special == 1 || c->special == 2) {
-        sws_rgb24_shuffle_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dstStride[0], dstFrame[0], w, h, c->special == 2);
-        return check_launch("sws_scale:rgb24 shuffle");
-    }
-    if (c->special >= 3) {
-        if (dstStride[1] != dstStride[2]) { set_error_msg("sws_scale", "packed -> yuv420p needs equal chroma pitches"); return -1; }
-        if (c->special >= 6) {
-            sws_yuyv_yuv422p_kernel<<<dim3(((w + 1) / 2 + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dst[1], dst[2], dstStride[0], dstStride[1],
-                                                                                            dstFrame[0], dstFrame[1], dstFrame[2], w, h, c->special == 7);
-        } else if (c->special == 3) {
-            if (w >> 1) sws_bgr24_yv12_kernel<<<dim3(((w >> 1) + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dst[1], dst[2], dstStride[0], dstStride[1],
-                                                                                                    dstFrame[0], dstFrame[1], dstFrame[2], w, h);
-        } else {
-            sws_yuyv_yv12_kernel<<<dim3(((w + 1) / 2 + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dst[1], dst[2], dstStride[0], dstStride[1],
-                                                                                         dstFrame[0], dstFrame[1], dstFrame[2], w, h, c->special == 5);
-        }
-        return check_launch("sws_scale:packed -> planar");
-    }
-    const int yPitch = (w + 15) & ~15, cPitch = (p.chrSrcW + 15) & ~15;
-    const size_t yPlane = (size_t)yPitch * h, cPlane = (size_t)cPitch * p.chrSrcH, need = (yPlane + 2 * cPlane) * nframes;
-    if (c->nv_bytes < need) {
-        AVB_CUDA(cudaStreamSynchronize(st), "sws_scale:reader");       // an earlier batch may still read the old planes
-        cudaFree(c->d_nv); c->d_nv = nullptr; c->nv_bytes = 0;
-        AVB_CUDA(cudaMalloc(&c->d_nv, need), "sws_scale:reader");
-        c->nv_bytes = need;
-    }
-    uint8_t *Y = c->d_nv, *U = Y + yPlane * nframes, *V = U + cPlane * nframes;
-    const dim3 grid(((w + 1) / 2 + 255) / 256, h, nframes);
-    const int half = p.chrSrcW != w;
-    if (c->srcPacked == 5) {
-        if (!src[1]) { set_error_msg("sws_scale", "pal8 source without a palette in plane 1"); return -1; }
-        sws_read_pal8_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], src[1], srcFrame[1], Y, U, V, yPitch, yPlane, w, h);
-    } else if (c->srcPacked == 1)      sws_read_packed_kernel<1><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, c->pkR, c->pkG, c->pkB, half);
-    else if (c->srcPacked == 4) sws_read_packed_kernel<4><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, c->pkR, c->pkG, c->pkB, half);
-    else if (c->srcPacked == 2) sws_read_packed_kernel<2><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, 0, 0, 0, 1);
-    else                        sws_read_packed_kernel<3><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, 0, 0, 0, 1);
-    if (check_launch("sws_scale:reader")) return -1;
-    const uint8_t *s3[3] = { Y, U, V };
-    const int st3[3] = { yPitch, cPitch, cPitch };
-    const size_t fr3[3] = { yPlane, cPlane, cPlane };
-    return run_planar(c, s3, st3, fr3, dst, dstStride, dstFrame, nframes, st);
+    const SwsGeometry &g = c->g;
+    if (is_packed_src(c->S)) return { 1, { (size_t)g.srcW * c->S->bpp, 0, 0 }, { g.srcH, 0, 0 } };
+    const size_t s = c->srcFmt->bits > 8 ? 2 : 1, nv = c->S->fam == FAM_NV;
+    return { nv ? 2 : 3, { g.srcW * s, g.chrSrcW * (nv ? 2 : 1) * s, g.chrSrcW * s }, { g.srcH, g.chrSrcH, g.chrSrcH } };
+}
+static PlaneGeom dst_planes(const SwsCudaContext *c)
+{
+    const SwsGeometry &g = c->g;
+    if (!is_planar(c->D)) return { 1, { (size_t)g.dstW * c->D->bpp, 0, 0 }, { g.dstH, 0, 0 } };
+    const size_t s = c->D->bits > 8 ? 2 : 1, nv = c->D->fam == FAM_NV;
+    return { nv ? 2 : 3, { g.dstW * s, g.chrDstW * (nv ? 2 : 1) * s, g.chrDstW * s }, { g.dstH, g.chrDstH, g.chrDstH } };
 }
 
-// the reference's nv12ToPlanarWrapper (swscale_unscaled.c:160-181): luma copy + a split of srcW/2 x srcH/2 samples.
-static int run_frames_24(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
-                         uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st,
-                         uint8_t *const *remapped = nullptr);
-
-// 32-bit rgb destinations: the rgb24 pipeline into a scratch picture, then one expansion pass (+ 6 B per pixel of traffic; fusing the
-// 4-byte store into every output kernel is the next step for this format family)
-static int run_frames(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
-                      uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st)
+// The planar -> packed 4:2:2 converters' pair count over a row of width w: the reference's 64-bit loop converts two pairs per step
+// (rgb2rgb_template.c:374-386), so an odd pair count is rounded up and the extra pair reads / writes past the nominal width --
+// reproduced when every row involved has room for it
+static int to422_pairs(int w, int dstStride, const int srcStride[3])
 {
-    if (!c->dst32 || c->special == 8 || c->special == 9 || c->special == 10) return run_frames_24(c, src, srcStride, srcFrame, dst, dstStride, dstFrame, nframes, st);      // (special 8: the rgb2rgb remap writes 4-byte pixels itself)
-    if (nframes <= 0) return 0;
-    const SwsDev &p = c->dev;
-    const int pitch = ((p.dstW + 1) * 3 + 15) & ~15;
-    const size_t frame = (size_t)pitch * p.dstH, need = frame * nframes;
-    if (c->rgb_bytes < need) {
-        AVB_CUDA(cudaStreamSynchronize(st), "sws_scale:rgb32");
-        cudaFree(c->d_rgb); c->d_rgb = nullptr; c->rgb_bytes = 0;
-        AVB_CUDA(cudaMalloc(&c->d_rgb, need), "sws_scale:rgb32");
-        c->rgb_bytes = need;
-    }
-    uint8_t *const d3[3] = { c->d_rgb, nullptr, nullptr };
-    const int s3[3] = { pitch, 0, 0 };
-    const size_t f3[3] = { frame, 0, 0 };
-    if (run_frames_24(c, src, srcStride, srcFrame, d3, s3, f3, nframes, st)) return -1;
-    // what the 24-bit functions write: whole pixel pairs (one pixel past an odd width when the row has room), single pixels with
-    // SWS_FULL_CHR_H_INT, and the unscaled table converter leaves an odd last column alone
-    int w = p.dstW;
-    if (c->table_unscaled) w &= ~1;
-    else if ((w & 1) && !p.full && dstStride[0] >= 4 * (w + 1)) w++;
-    static const int order[4][4] = { { 1, 2, 3, 0 }, { 0, 1, 2, 3 }, { 3, 2, 1, 0 }, { 2, 1, 0, 3 } };    // argb, rgba, abgr, bgra: r g b a positions
-    const int *o = order[c->dst32 - FMT_ARGB];
-    sws_expand_rgb32_kernel<<<dim3((w + 255) / 256, p.dstH, nframes), 256, 0, st>>>(c->d_rgb, pitch, frame, dst[0], dstStride[0], dstFrame[0], w, o[0], o[1], o[2], o[3]);
-    return check_launch("sws_scale:rgb32");
+    const int pairs = w >> 1, pairs_r = (pairs + 1) & ~1;
+    return pairs_r > pairs && dstStride >= 4 * pairs_r && srcStride[0] >= 2 * pairs_r && srcStride[1] >= pairs_r && srcStride[2] >= pairs_r ? pairs_r : pairs;
 }
 
-static int run_frames_24(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
-                         uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st,
-                         uint8_t *const *remapped)
+// The pixels of each packed destination row the route writes
+static int packed_cols(const SwsCudaContext *c, int dstStride, const int srcStride[3])
 {
-    if (c->special == 10) {            // pal8 -> 24 / 32-bit rgb of the same size: the palette lookup of palToRgbWrapper
-        if (nframes <= 0) return 0;
-        if (!src[1]) { set_error_msg("sws_scale", "pal8 source without a palette in plane 1"); return -1; }
-        static const int chan[6][4] = { { 0, 1, 2, -1 }, { 2, 1, 0, -1 }, { 1, 2, 3, 0 }, { 0, 1, 2, 3 }, { 3, 2, 1, 0 }, { 2, 1, 0, 3 } };      // byte of r, g, b, a
-        const SwsDev &q = c->dev;
-        const int df = c->dst32 ? 2 + c->dst32 - FMT_ARGB : c->dstFormat == FMT_BGR24 ? 1 : 0, dbpp = c->dst32 ? 4 : 3;
-        unsigned map = 0;
-        for (int ch = 0; ch < 4; ch++) if (chan[df][ch] >= 0) map |= (unsigned)(ch < 3 ? ch : 15) << (4 * chan[df][ch]);
-        sws_pal8_rgb_kernel<<<dim3((q.srcW + 255) / 256, q.srcH, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], src[1], srcFrame[1], dst[0], dstStride[0], dstFrame[0],
-                                                                                     q.srcW, q.srcH, dbpp, map);
-        return check_launch("sws_scale:pal8 -> rgb");
+    const int w = c->g.dstW;
+    switch (c->route) {
+    case R_TABLE: return w & ~1;                            // the unscaled table converter leaves an odd last column alone
+    case R_422_FROM_422P: case R_422_FROM_420P: return 2 * to422_pairs(w, dstStride, srcStride);
+    case R_SCALE: case R_FUSED: case R_RGB48:               // whole pixel pairs, one pixel past an odd width when the row has room; single
+        return (w & 1) && !c->dev.full && dstStride >= (w + 1) * c->D->bpp ? w + 1 : w;        // pixels with SWS_FULL_CHR_H_INT
+    default: return w;
     }
-    if (c->special == 9) {             // gray8 -> 24 / 32-bit rgb of the same size: the pseudo-palette lookup is r = g = b = sample, alpha 255
-        if (nframes <= 0) return 0;
-        const SwsDev &q = c->dev;
-        const int dbpp = c->dst32 ? 4 : 3;
-        const unsigned map = !c->dst32 ? 0x000u : (c->dst32 == FMT_ARGB || c->dst32 == FMT_ABGR) ? 0x000Fu : 0xF000u;
-        sws_rgb_map_kernel<<<dim3((q.srcW + 255) / 256, q.srcH, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dstStride[0], dstFrame[0], q.srcW, q.srcH, 1, dbpp, map);
-        return check_launch("sws_scale:gray8 -> rgb");
-    }
-    if (c->to422) {
-        const SwsDev &q = c->dev;
-        if (nframes <= 0) return 0;
-        if (c->to422 == 3) {
-            for (int f = 0; f < nframes; f++)
-                AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], (size_t)q.srcW * 2, q.srcH, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
-            return 0;
-        }
-        if (srcStride[1] != srcStride[2]) { set_error_msg("sws_scale", "planar -> packed 4:2:2 needs equal chroma pitches"); return -1; }
-        // the reference's 64-bit loop converts two pairs per step (rgb2rgb_template.c:374-386): an odd pair count is rounded up and the extra
-        // pair reads / writes past the nominal width -- reproduced when every row involved has room for it
-        const int pairs = q.srcW >> 1, pairs_r = (pairs + 1) & ~1;
-        const bool extra = pairs_r > pairs && dstStride[0] >= 4 * pairs_r && srcStride[0] >= 2 * pairs_r && srcStride[1] >= pairs_r;
-        const int np = extra ? pairs_r : pairs;
-        if (np)
-            sws_planar_to_422_kernel<<<dim3((np + 255) / 256, q.srcH, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], src[1], src[2], srcStride[1], srcFrame[1], srcFrame[2],
-                                                                                          dst[0], dstStride[0], dstFrame[0], 2 * np, c->to422 == 2 ? 1 : 0, c->pk422 == 2);
-        return check_launch("sws_scale:planar -> packed 4:2:2");
-    }
-    if (c->dstNV && !remapped) {       // an nv12 / nv21 destination: U and V are the even / odd bytes of plane 1 (chrStep 2 in the kernels)
-        if (c->nvcopy) {
-            const SwsDev &q = c->dev;
-            if (nframes <= 0) return 0;
-            for (int f = 0; f < nframes; f++)
-                AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], q.srcW, q.srcH, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
-            const int sw = c->dstNV == 2;
-            if (q.srcW / 2 > 0 && q.srcH / 2 > 0)
-                sws_interleave_kernel<<<dim3((q.srcW / 2 + 255) / 256, q.srcH / 2, nframes), 256, 0, st>>>(src[sw ? 2 : 1], srcStride[sw ? 2 : 1], srcFrame[sw ? 2 : 1], src[sw ? 1 : 2],
-                                                                                                     srcStride[sw ? 1 : 2], srcFrame[sw ? 1 : 2], dst[1], dstStride[1], dstFrame[1], q.srcW / 2);
-            return check_launch("sws_scale:planar -> nv12");
-        }
-        uint8_t *const d3[3] = { dst[0], dst[1] + (c->dstNV == 2 ? 1 : 0), dst[1] + (c->dstNV == 2 ? 0 : 1) };
-        const int s3[3] = { dstStride[0], dstStride[1], dstStride[1] };
-        const size_t f3[3] = { dstFrame[0], dstFrame[1], dstFrame[1] };
-        return run_frames_24(c, src, srcStride, srcFrame, d3, s3, f3, nframes, st, d3);
-    }
-    if (c->srcPacked) return run_packed(c, src, srcStride, srcFrame, dst, dstStride, dstFrame, nframes, st);
-    if (!c->srcNV) return run_planar(c, src, srcStride, srcFrame, dst, dstStride, dstFrame, nframes, st);
-    if (nframes <= 0) return 0;
-    const SwsDev &p = c->dev;
-    const int swap = c->srcNV == 2;
-    if (c->copy) {
-        const int w = p.srcW / 2, h = p.srcH / 2;
-        for (int f = 0; f < nframes; f++)
-            AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], p.srcW, p.srcH,
-                                       cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
-        if (w > 0 && h > 0) {
-            if (dstStride[1] != dstStride[2]) { set_error_msg("sws_scale", "nv12 -> planar copy needs equal chroma pitches"); return -1; }
-            sws_split_nv_kernel<<<dim3((w + 1023) / 1024, h, nframes), 256, 0, st>>>(src[1], srcStride[1], srcFrame[1], dst[swap ? 2 : 1], dst[swap ? 1 : 2],
-                                                                                 dstStride[1], dstFrame[swap ? 2 : 1], dstFrame[swap ? 1 : 2], w, h);
-        }
-        return check_launch("sws_scale:nv12 copy");
-    }
-    const int pitch = (p.chrSrcW + 15) & ~15;
-    const size_t plane = (size_t)pitch * p.chrSrcH, need = 2 * plane * nframes;
-    if (c->nv_bytes < need) {
-        AVB_CUDA(cudaStreamSynchronize(st), "sws_scale:nv12");         // an earlier batch may still read the old planes
-        cudaFree(c->d_nv); c->d_nv = nullptr; c->nv_bytes = 0;
-        AVB_CUDA(cudaMalloc(&c->d_nv, need), "sws_scale:nv12");
-        c->nv_bytes = need;
-    }
-    uint8_t *U = c->d_nv, *V = c->d_nv + plane * nframes;
-    sws_split_nv_kernel<<<dim3((p.chrSrcW + 1023) / 1024, p.chrSrcH, nframes), 256, 0, st>>>(src[1], srcStride[1], srcFrame[1], swap ? V : U, swap ? U : V,
-                                                                                          pitch, plane, plane, p.chrSrcW, p.chrSrcH);
-    if (check_launch("sws_scale:nv12 split")) return -1;
-    const uint8_t *s3[3] = { src[0], U, V };
-    const int st3[3] = { srcStride[0], pitch, pitch };
-    const size_t fr3[3] = { srcFrame[0], plane, plane };
-    return run_planar(c, s3, st3, fr3, dst, dstStride, dstFrame, nframes, st);
+}
+
+// The samples of each planar destination plane the route writes: luma columns; chroma columns and rows
+static void planar_extent(const SwsCudaContext *c, int &w, int &cw, int &ch)
+{
+    const SwsGeometry &g = c->g;
+    const bool nvSplit = c->route == R_COPY && c->S->fam == FAM_NV;
+    w = c->route == R_BGR24_YV12 ? g.dstW & ~1 : g.dstW;     // rgb24toyv12_c converts whole pixel pairs only
+    // nv12ToPlanarWrapper and planarToNv12Wrapper move srcW / 2 x srcH / 2 chroma samples: an odd last column / row stays untouched;
+    // the packed -> yuv420p converters write srcH / 2 chroma rows
+    cw = nvSplit || c->route == R_BGR24_YV12 || c->route == R_NV_INTERLEAVE ? g.srcW / 2 : g.chrDstW;
+    ch = nvSplit || c->route == R_BGR24_YV12 || c->route == R_YUYV_420P || c->route == R_NV_INTERLEAVE ? g.srcH / 2 : g.chrDstH;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// dispatch
+// ---------------------------------------------------------------------------------------------------
+static FusedArgs fused_args(const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3], uint8_t *dst, int dstStride, size_t dstFrame)
+{
+    FusedArgs a;
+    a.y = src[0]; a.u = src[1]; a.v = src[2]; a.dst = dst;
+    a.yStride = srcStride[0]; a.uStride = srcStride[1]; a.vStride = srcStride[2]; a.dstStride = dstStride;
+    a.yFrame = srcFrame[0]; a.uFrame = srcFrame[1]; a.vFrame = srcFrame[2]; a.dstFrame = dstFrame;
+    return a;
 }
 
 // the interior fast path of the fused same-size kernel over row pairs [a.rp0, a.rp1): TMA-staged (sws_fused_tma.cu) when tensor maps can
@@ -1976,79 +1864,40 @@ static int launch_fused_fast(SwsCudaContext *c, const FusedArgs &a, int nframes,
     return check_launch("sws_scale:fused");
 }
 
-static int run_planar(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
-                      uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st)
+static int run_fused(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
+                     uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st)
 {
     const SwsDev &p = c->dev;
-    if (nframes <= 0) return 0;
-    if (c->copy && p.dstBits != 8) {
-        for (int pl = 0; pl < 3; pl++) {
-            const int w = pl ? p.chrSrcW : p.srcW, h = pl ? p.chrSrcH : p.srcH;
-            sws_copy_plane_up_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[pl], srcStride[pl], srcFrame[pl], dst[pl], dstStride[pl], dstFrame[pl], w, h, p.dstBits - 8, p.dstBE);
-        }
-        return check_launch("sws_scale:copy");
+    FusedArgs a = fused_args(src, srcStride, srcFrame, dst[0], dstStride[0], dstFrame[0]);
+    // vector accesses need 8-byte aligned luma / output rows and 4-byte aligned chroma rows
+    bool aligned = !((uintptr_t)a.y & 7) && !(a.yStride & 7) && !((uintptr_t)a.dst & 7) && !(a.dstStride & 7) && !(a.yFrame & 7) &&
+                   !(a.dstFrame & 7) && !((uintptr_t)a.u & 3) && !((uintptr_t)a.v & 3) && !(a.uStride & 3) && !(a.vStride & 3) &&
+                   !(a.uFrame & 3) && !(a.vFrame & 3);
+    const bool a16 = aligned && !((uintptr_t)a.y & 15) && !(a.yStride & 15) && !((uintptr_t)a.dst & 15) && !(a.dstStride & 15) &&
+                     !(a.yFrame & 15) && !(a.dstFrame & 15) && !((uintptr_t)a.u & 7) && !((uintptr_t)a.v & 7) && !(a.uStride & 7) &&
+                     !(a.vStride & 7) && !(a.uFrame & 7) && !(a.vFrame & 7) && !((uintptr_t)p.vChrF & 15);
+    if (c->fast_ok && a16 && tuning("sws_fused_variant") != 1) {
+        a.rp0 = 0; a.rp1 = p.dstH / 2;
+        return launch_fused_fast(c, a, nframes, st);
     }
-    if (c->copy && c->srcGray) {       // planarCopyWrapper for a gray source: the luma plane, and 128 in the planes the source does not have (swscale_unscaled.c:812-823)
-        for (int f = 0; f < nframes; f++) {
-            AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], p.srcW, p.srcH, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
-            for (int pl = 1; pl < 3; pl++)
-                AVB_CUDA(cudaMemset2DAsync(dst[pl] + f * dstFrame[pl], dstStride[pl], 128, p.chrDstW, p.chrDstH, st), "sws_scale:copy");
-        }
-        return 0;
-    }
-    if (c->copy) {
-        for (int f = 0; f < nframes; f++)
-            for (int pl = 0; pl < 3; pl++) {
-                int w = pl ? p.chrSrcW : p.srcW, h = pl ? p.chrSrcH : p.srcH;
-                AVB_CUDA(cudaMemcpy2DAsync(dst[pl] + f * dstFrame[pl], dstStride[pl], src[pl] + f * srcFrame[pl], srcStride[pl], w, h,
-                                           cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
-            }
-        return 0;
-    }
-    if (c->table_unscaled) {
-        FusedArgs a;
-        a.y = src[0]; a.u = src[1]; a.v = src[2]; a.dst = dst[0];
-        a.yStride = srcStride[0]; a.uStride = srcStride[1] << (c->src422 ? 1 : 0); a.vStride = srcStride[2] << (c->src422 ? 1 : 0); a.dstStride = dstStride[0];
-        a.yFrame = srcFrame[0]; a.uFrame = srcFrame[1]; a.vFrame = srcFrame[2]; a.dstFrame = dstFrame[0];
-        sws_unscaled_yuv2rgb24_kernel<<<dim3(((p.dstW >> 1) + 255) / 256, p.dstH >> 1, nframes), 256, 0, st>>>(p, a);
-        return check_launch("sws_scale:unscaled");
-    }
-    if (c->rgb48) {
-        FusedArgs a;
-        a.y = src[0]; a.u = src[1]; a.v = src[2]; a.dst = dst[0];
-        a.yStride = srcStride[0]; a.uStride = srcStride[1]; a.vStride = srcStride[2]; a.dstStride = dstStride[0];
-        a.yFrame = srcFrame[0]; a.uFrame = srcFrame[1]; a.vFrame = srcFrame[2]; a.dstFrame = dstFrame[0];
-        sws_rgb48_kernel<<<dim3((((p.dstW + 1) >> 1) + 127) / 128, p.dstH, nframes), 128, 0, st>>>(p, a);
-        return check_launch("sws_scale:rgb48");
-    }
-    if (c->fused) {
-        FusedArgs a;
-        a.y = src[0]; a.u = src[1]; a.v = src[2]; a.dst = dst[0];
-        a.yStride = srcStride[0]; a.uStride = srcStride[1]; a.vStride = srcStride[2]; a.dstStride = dstStride[0];
-        a.yFrame = srcFrame[0]; a.uFrame = srcFrame[1]; a.vFrame = srcFrame[2]; a.dstFrame = dstFrame[0];
-        // vector accesses need 8-byte aligned luma / output rows and 4-byte aligned chroma rows
-        bool aligned = !((uintptr_t)a.y & 7) && !(a.yStride & 7) && !((uintptr_t)a.dst & 7) && !(a.dstStride & 7) && !(a.yFrame & 7) &&
-                       !(a.dstFrame & 7) && !((uintptr_t)a.u & 3) && !((uintptr_t)a.v & 3) && !(a.uStride & 3) && !(a.vStride & 3) &&
-                       !(a.uFrame & 3) && !(a.vFrame & 3);
-        const bool a16 = aligned && !((uintptr_t)a.y & 15) && !(a.yStride & 15) && !((uintptr_t)a.dst & 15) && !(a.dstStride & 15) &&
-                         !(a.yFrame & 15) && !(a.dstFrame & 15) && !((uintptr_t)a.u & 7) && !((uintptr_t)a.v & 7) && !(a.uStride & 7) &&
-                         !(a.vStride & 7) && !(a.uFrame & 7) && !(a.vFrame & 7) && !((uintptr_t)p.vChrF & 15);
-        if (c->fast_ok && a16 && tuning("sws_fused_variant") != 1) {
-            a.rp0 = 0; a.rp1 = p.dstH / 2;
-            return launch_fused_fast(c, a, nframes, st);
-        }
-        dim3 b(32, 8), g((p.dstW + 255) / 256, (p.dstH + 15) / 16, nframes);
-        if (aligned) sws_fused_rgb24_kernel<true><<<g, b, 0, st>>>(p, a);
-        else         sws_fused_rgb24_kernel<false><<<g, b, 0, st>>>(p, a);    // same arithmetic, byte accesses
-        return check_launch("sws_scale:fused");
-    }
+    dim3 b(32, 8), g((p.dstW + 255) / 256, (p.dstH + 15) / 16, nframes);
+    if (aligned) sws_fused_rgb24_kernel<true><<<g, b, 0, st>>>(p, a);
+    else         sws_fused_rgb24_kernel<false><<<g, b, 0, st>>>(p, a);    // same arithmetic, byte accesses
+    return check_launch("sws_scale:fused");
+}
+
+// the general scaler: fused per output tile when the vertical windows fit in shared memory, else two passes over line planes
+static int run_scale(SwsCudaContext *c, const uint8_t *const src[3], const int srcStride[3], const size_t srcFrame[3],
+                     uint8_t *const dst[3], const int dstStride[3], const size_t dstFrame[3], int nframes, cudaStream_t st)
+{
+    const SwsDev &p = c->dev;
+    const bool planar = is_planar(c->D);
     if (c->tileLumRows && (tuning("sws_general_variant") != 1 || p.dstBits == 16)) {       // general path, fused per output tile
         TileArgs a;
         a.y = src[0]; a.u = src[1]; a.v = src[2]; a.dst0 = dst[0]; a.dst1 = dst[1]; a.dst2 = dst[2];
         a.yStride = srcStride[0]; a.uStride = srcStride[1]; a.vStride = srcStride[2];
         a.yFrame = srcFrame[0]; a.uFrame = srcFrame[1]; a.vFrame = srcFrame[2];
         a.dstStride0 = dstStride[0]; a.dstFrame0 = dstFrame[0];
-        const bool planar = c->planar;
         a.dstStride1 = planar ? dstStride[1] : 0; a.dstStride2 = planar ? dstStride[2] : 0;
         a.dstFrame1 = planar ? dstFrame[1] : 0; a.dstFrame2 = planar ? dstFrame[2] : 0;
         a.lumRows = c->tileLumRows; a.chrRows = c->tileChrRows;
@@ -2095,7 +1944,7 @@ static int run_planar(SwsCudaContext *c, const uint8_t *const src[3], const int 
     for (int f = 0; f < nframes; f++) {      // general path, two passes: frames are serialised on the stream (shared line planes)
         const uint8_t *y = src[0] + f * srcFrame[0], *u = src[1] + f * srcFrame[1], *v = src[2] + f * srcFrame[2];
         dim3 b(256);
-        if (c->srcGray) {                     // luma only; the chroma lines keep the bytes of 64 sws_init_context wrote (0x4040 per 15-bit sample)
+        if (p.srcGray) {                     // luma only; the chroma lines keep the bytes of 64 sws_init_context wrote (0x4040 per 15-bit sample)
             if (c->g.flags & SWS_FAST_BILINEAR)
                 sws_hscale_fast_kernel<<<dim3((p.dstW + 255) / 256, p.srcH), b, 0, st>>>(y, srcStride[0], c->d_lum, c->lumStridePx, p.srcW, p.dstW, p.srcH, c->g.lumXInc, 0);
             else
@@ -2120,7 +1969,7 @@ static int run_planar(SwsCudaContext *c, const uint8_t *const src[3], const int 
                 sws_launch_range(c->d_chrU, c->chrStridePx, p.chrDstW, p.chrSrcH, c->rangeConv == 1 ? 1 : 3, st) ||
                 sws_launch_range(c->d_chrV, c->chrStridePx, p.chrDstW, p.chrSrcH, c->rangeConv == 1 ? 1 : 3, st)) return -1;
         }
-        if (c->planar) {
+        if (planar) {
             sws_vscale_plane_kernel<<<dim3((p.dstW + 255) / 256, p.dstH), b, 0, st>>>(c->d_lum, c->lumStridePx, p.srcH, p.vLumF, p.vLumP, p.vLumSize, dst[0] + f * dstFrame[0], dstStride[0], p.dstW, p.dstH, p.dstBits, p.dstBE, 1, p.dither, 0);
             sws_vscale_plane_kernel<<<dim3((p.chrDstW + 255) / 256, p.chrDstH), b, 0, st>>>(c->d_chrU, c->chrStridePx, p.chrSrcH, p.vChrF, p.vChrP, p.vChrSize, dst[1] + f * dstFrame[1], dstStride[1], p.chrDstW, p.chrDstH, p.dstBits, p.dstBE, p.chrStep, p.dither, 0);
             sws_vscale_plane_kernel<<<dim3((p.chrDstW + 255) / 256, p.chrDstH), b, 0, st>>>(c->d_chrV, c->chrStridePx, p.chrSrcH, p.vChrF, p.vChrP, p.vChrSize, dst[2] + f * dstFrame[2], dstStride[2], p.chrDstW, p.chrDstH, p.dstBits, p.dstBE, p.chrStep, p.dither, 3);      // chrDither8 with offset 3 for V (swscale.c:636-644)
@@ -2142,14 +1991,189 @@ static int run_planar(SwsCudaContext *c, const uint8_t *const src[3], const int 
     return 0;
 }
 
+// byte map of sws_rgb_map_kernel / sws_pal8_rgb_kernel: destination byte i of a pixel takes source byte (map >> 4 i) & 15, 15 = 255.
+// from[] holds the source byte of r, g, b and a (-1: none)
+static unsigned channel_map(const PixFmt *d, const int (&from)[4])
+{
+    const int to[4] = { d->r, d->g, d->b, d->a };
+    unsigned map = 0;
+    for (int ch = 0; ch < 4; ch++) if (to[ch] >= 0) map |= (unsigned)(from[ch] >= 0 ? from[ch] : 15) << (4 * to[ch]);
+    return map;
+}
+
+// One batch of frames on device pointers: the source pre-pass, the route, the 32-bit expansion.  src[] / dst[] are the planes the
+// route reads and writes (for gray8 the public entry points substituted them).
+static int run_frames(SwsCudaContext *c, const uint8_t *const src_[3], const int srcStride_[3], const size_t srcFrame_[3],
+                      uint8_t *const dst_[3], const int dstStride_[3], const size_t dstFrame_[3], int nframes, cudaStream_t st)
+{
+    if (nframes <= 0) return 0;
+    const SwsDev &p = c->dev;
+    const PixFmt *S = c->S, *D = c->D;
+    const Route r = c->route;
+    const int w = p.srcW, h = p.srcH;
+    const uint8_t *src[3] = { src_[0], src_[1], src_[2] };
+    int srcStride[3] = { srcStride_[0], srcStride_[1], srcStride_[2] };
+    size_t srcFrame[3] = { srcFrame_[0], srcFrame_[1], srcFrame_[2] };
+    uint8_t *dst[3] = { dst_[0], dst_[1], dst_[2] };
+    int dstStride[3] = { dstStride_[0], dstStride_[1], dstStride_[2] };
+    size_t dstFrame[3] = { dstFrame_[0], dstFrame_[1], dstFrame_[2] };
+    if (D->fam == FAM_NV && r != R_NV_INTERLEAVE) {      // U and V are the even / odd bytes of plane 1 (chrStep 2 in the kernels)
+        const int v = D->fmt == PIX_NV21;
+        dst[2] = dst_[1] + (v ? 0 : 1); dst[1] = dst_[1] + v;
+        dstStride[2] = dstStride[1]; dstFrame[2] = dstFrame[1];
+    }
+    // 32-bit rgb destinations: the rgb24 pipeline into a scratch picture, then one expansion pass (+ 6 B per pixel of traffic; fusing the
+    // 4-byte store into every output kernel is the next step for this format family)
+    const bool expand = D->fam == FAM_RGB32 && ROUTES[r].planar;
+    const int pitch32 = ((p.dstW + 1) * 3 + 15) & ~15;
+    const size_t frame32 = (size_t)pitch32 * p.dstH;
+    if (expand) {
+        if (grow(c->d_rgb, c->rgb_bytes, frame32 * nframes, st, "sws_scale:rgb32")) return -1;
+        dst[0] = c->d_rgb; dst[1] = dst[2] = nullptr;
+        dstStride[0] = pitch32; dstStride[1] = dstStride[2] = 0;
+        dstFrame[0] = frame32; dstFrame[1] = dstFrame[2] = 0;
+    }
+    if (ROUTES[r].planar && S->fam == FAM_NV) {      // semi-planar sources: split the interleaved chroma plane (input.c:475-497)
+        const int pitch = (p.chrSrcW + 15) & ~15, swap = S->fmt == PIX_NV21;
+        const size_t plane = (size_t)pitch * p.chrSrcH;
+        if (grow(c->d_nv, c->nv_bytes, 2 * plane * nframes, st, "sws_scale:nv12")) return -1;
+        uint8_t *U = c->d_nv, *V = c->d_nv + plane * nframes;
+        sws_split_nv_kernel<<<dim3((p.chrSrcW + 1023) / 1024, p.chrSrcH, nframes), 256, 0, st>>>(src[1], srcStride[1], srcFrame[1], swap ? V : U, swap ? U : V,
+                                                                                              pitch, plane, plane, p.chrSrcW, p.chrSrcH);
+        if (check_launch("sws_scale:nv12 split")) return -1;
+        src[1] = U; src[2] = V; srcStride[1] = srcStride[2] = pitch; srcFrame[1] = srcFrame[2] = plane;
+    } else if (ROUTES[r].planar && is_packed_src(S)) {
+        // packed sources: the input readers (input.c) into planes, + srcW * srcH * (1 + 2 / 2^hs) bytes written and read again
+        const int yPitch = (w + 15) & ~15, cPitch = (p.chrSrcW + 15) & ~15;
+        const size_t yPlane = (size_t)yPitch * h, cPlane = (size_t)cPitch * p.chrSrcH;
+        if (grow(c->d_nv, c->nv_bytes, (yPlane + 2 * cPlane) * nframes, st, "sws_scale:reader")) return -1;
+        uint8_t *Y = c->d_nv, *U = Y + yPlane * nframes, *V = U + cPlane * nframes;
+        const dim3 grid(((w + 1) / 2 + 255) / 256, h, nframes);
+        const int half = p.chrSrcW != w;
+        if (S->fam == FAM_PAL8) {
+            if (!src[1]) { set_error_msg("sws_scale", "pal8 source without a palette in plane 1"); return -1; }
+            sws_read_pal8_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], src[1], srcFrame[1], Y, U, V, yPitch, yPlane, w, h);
+        } else if (S->fam == FAM_RGB24) sws_read_packed_kernel<1><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, S->r, S->g, S->b, half);
+        else if (S->fam == FAM_RGB32)   sws_read_packed_kernel<4><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, S->r, S->g, S->b, half);
+        else if (S->pk422 == 1)         sws_read_packed_kernel<2><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, 0, 0, 0, 1);
+        else                            sws_read_packed_kernel<3><<<grid, 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], Y, U, V, yPitch, cPitch, yPlane, cPlane, w, h, 0, 0, 0, 1);
+        if (check_launch("sws_scale:reader")) return -1;
+        src[0] = Y; src[1] = U; src[2] = V;
+        srcStride[0] = yPitch; srcStride[1] = srcStride[2] = cPitch;
+        srcFrame[0] = yPlane; srcFrame[1] = srcFrame[2] = cPlane;
+    }
+    switch (r) {
+    case R_PAL8_RGB: {             // the palette lookup of palToRgbWrapper
+        if (!src[1]) { set_error_msg("sws_scale", "pal8 source without a palette in plane 1"); return -1; }
+        sws_pal8_rgb_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], src[1], srcFrame[1], dst[0], dstStride[0], dstFrame[0],
+                                                                            w, h, D->bpp, channel_map(D, { 0, 1, 2, -1 }));
+        return check_launch("sws_scale:pal8 -> rgb");
+    }
+    case R_GRAY_RGB:               // the pseudo-palette lookup is r = g = b = sample, alpha 255
+        sws_rgb_map_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dstStride[0], dstFrame[0], w, h, 1, D->bpp, channel_map(D, { 0, 0, 0, -1 }));
+        return check_launch("sws_scale:gray8 -> rgb");
+    case R_RGB_REMAP:
+        sws_rgb_map_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dstStride[0], dstFrame[0], w, h, S->bpp, D->bpp,
+                                                                           channel_map(D, { S->r, S->g, S->b, S->a }));
+        return check_launch("sws_scale:rgb2rgb");
+    case R_RGB_COPY: case R_RGB24_SWAP:
+        sws_rgb24_shuffle_kernel<<<dim3((w + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dstStride[0], dstFrame[0], w, h, r == R_RGB24_SWAP);
+        return check_launch("sws_scale:rgb24 shuffle");
+    case R_BGR24_YV12: case R_YUYV_420P: case R_YUYV_422P:
+        if (dstStride[1] != dstStride[2]) { set_error_msg("sws_scale", "packed -> yuv420p needs equal chroma pitches"); return -1; }
+        if (r == R_YUYV_422P) {
+            sws_yuyv_yuv422p_kernel<<<dim3(((w + 1) / 2 + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dst[1], dst[2], dstStride[0], dstStride[1],
+                                                                                            dstFrame[0], dstFrame[1], dstFrame[2], w, h, S->pk422 == 2);
+        } else if (r == R_BGR24_YV12) {
+            if (w >> 1) sws_bgr24_yv12_kernel<<<dim3(((w >> 1) + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dst[1], dst[2], dstStride[0], dstStride[1],
+                                                                                                    dstFrame[0], dstFrame[1], dstFrame[2], w, h);
+        } else {
+            sws_yuyv_yv12_kernel<<<dim3(((w + 1) / 2 + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], dst[0], dst[1], dst[2], dstStride[0], dstStride[1],
+                                                                                         dstFrame[0], dstFrame[1], dstFrame[2], w, h, S->pk422 == 2);
+        }
+        return check_launch("sws_scale:packed -> planar");
+    case R_422_COPY:
+        for (int f = 0; f < nframes; f++)
+            AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], (size_t)w * 2, h, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
+        return 0;
+    case R_422_FROM_422P: case R_422_FROM_420P: {
+        if (srcStride[1] != srcStride[2]) { set_error_msg("sws_scale", "planar -> packed 4:2:2 needs equal chroma pitches"); return -1; }
+        const int np = to422_pairs(w, dstStride[0], srcStride);
+        if (np)
+            sws_planar_to_422_kernel<<<dim3((np + 255) / 256, h, nframes), 256, 0, st>>>(src[0], srcStride[0], srcFrame[0], src[1], src[2], srcStride[1], srcFrame[1], srcFrame[2],
+                                                                                      dst[0], dstStride[0], dstFrame[0], 2 * np, r == R_422_FROM_420P, D->pk422 == 2);
+        return check_launch("sws_scale:planar -> packed 4:2:2");
+    }
+    case R_NV_INTERLEAVE: {
+        for (int f = 0; f < nframes; f++)
+            AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], w, h, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
+        const int u = D->fmt == PIX_NV21 ? 2 : 1, v = 3 - u;
+        if (w / 2 > 0 && h / 2 > 0)
+            sws_interleave_kernel<<<dim3((w / 2 + 255) / 256, h / 2, nframes), 256, 0, st>>>(src[u], srcStride[u], srcFrame[u], src[v], srcStride[v], srcFrame[v],
+                                                                                         dst[1], dstStride[1], dstFrame[1], w / 2);
+        return check_launch("sws_scale:planar -> nv12");
+    }
+    case R_COPY:
+        if (S->fam == FAM_NV) {        // nv12ToPlanarWrapper (swscale_unscaled.c:160-181): luma copy + a split of srcW/2 x srcH/2 samples
+            const int swap = S->fmt == PIX_NV21;
+            for (int f = 0; f < nframes; f++)
+                AVB_CUDA(cudaMemcpy2DAsync(dst[0] + f * dstFrame[0], dstStride[0], src[0] + f * srcFrame[0], srcStride[0], w, h, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
+            if (w / 2 > 0 && h / 2 > 0) {
+                if (dstStride[1] != dstStride[2]) { set_error_msg("sws_scale", "nv12 -> planar copy needs equal chroma pitches"); return -1; }
+                sws_split_nv_kernel<<<dim3((w / 2 + 1023) / 1024, h / 2, nframes), 256, 0, st>>>(src[1], srcStride[1], srcFrame[1], dst[swap ? 2 : 1], dst[swap ? 1 : 2],
+                                                                                             dstStride[1], dstFrame[swap ? 2 : 1], dstFrame[swap ? 1 : 2], w / 2, h / 2);
+            }
+            return check_launch("sws_scale:nv12 copy");
+        }
+        if (p.dstBits != 8) {
+            for (int pl = 0; pl < 3; pl++) {
+                const int pw = pl ? p.chrSrcW : w, ph = pl ? p.chrSrcH : h;
+                sws_copy_plane_up_kernel<<<dim3((pw + 255) / 256, ph, nframes), 256, 0, st>>>(src[pl], srcStride[pl], srcFrame[pl], dst[pl], dstStride[pl], dstFrame[pl], pw, ph, p.dstBits - 8, p.dstBE);
+            }
+            return check_launch("sws_scale:copy");
+        }
+        for (int f = 0; f < nframes; f++)
+            for (int pl = 0; pl < 3; pl++) {
+                // a gray source: the luma plane, and 128 in the planes the source does not have (swscale_unscaled.c:812-823)
+                if (pl && p.srcGray)
+                    AVB_CUDA(cudaMemset2DAsync(dst[pl] + f * dstFrame[pl], dstStride[pl], 128, p.chrDstW, p.chrDstH, st), "sws_scale:copy");
+                else
+                    AVB_CUDA(cudaMemcpy2DAsync(dst[pl] + f * dstFrame[pl], dstStride[pl], src[pl] + f * srcFrame[pl], srcStride[pl], pl ? p.chrSrcW : w,
+                                               pl ? p.chrSrcH : h, cudaMemcpyDeviceToDevice, st), "sws_scale:copy");
+            }
+        return 0;
+    case R_TABLE: {
+        FusedArgs a = fused_args(src, srcStride, srcFrame, dst[0], dstStride[0], dstFrame[0]);
+        if (!S->vs) { a.uStride <<= 1; a.vStride <<= 1; }    // a 4:2:2 source: the even chroma line serves both rows (yuv2rgb.c:133-136)
+        sws_unscaled_yuv2rgb24_kernel<<<dim3(((p.dstW >> 1) + 255) / 256, p.dstH >> 1, nframes), 256, 0, st>>>(p, a);
+        if (check_launch("sws_scale:unscaled")) return -1;
+        break;
+    }
+    case R_RGB48:
+        sws_rgb48_kernel<<<dim3((((p.dstW + 1) >> 1) + 127) / 128, p.dstH, nframes), 128, 0, st>>>(p, fused_args(src, srcStride, srcFrame, dst[0], dstStride[0], dstFrame[0]));
+        return check_launch("sws_scale:rgb48");
+    case R_FUSED:
+        if (run_fused(c, src, srcStride, srcFrame, dst, dstStride, dstFrame, nframes, st)) return -1;
+        break;
+    case R_SCALE:
+        if (run_scale(c, src, srcStride, srcFrame, dst, dstStride, dstFrame, nframes, st)) return -1;
+        break;
+    }
+    if (!expand) return 0;
+    const int cols = packed_cols(c, dstStride_[0], srcStride_);
+    sws_expand_rgb32_kernel<<<dim3((cols + 255) / 256, p.dstH, nframes), 256, 0, st>>>(c->d_rgb, pitch32, frame32, dst_[0], dstStride_[0], dstFrame_[0], cols, D->r, D->g, D->b, D->a);
+    return check_launch("sws_scale:rgb32");
+}
+
 bool sws_slot_view(const void *ctx, SwsSlotView &v)
 {
     const SwsCudaContext *c = (const SwsCudaContext *)ctx;
     if (!c) return false;
-    v.rangeConv = c->rangeConv; v.srcBits = c->srcBits;
-    v.k = c->k; v.flags = c->g.flags; v.planar = c->planar; v.dstBits = c->dstBits; v.dstBE = c->dstBE; v.dstNV = c->dstNV;
-    if (c->rgb16 || c->rgb48 || c->gray || c->srcGray) return false; // (the per-line slots do not cover the 15 / 16 / 12 / 48-bpp output stages: the hook leaves the C slots)
-    v.target = c->planar ? -1 : c->pk422 ? 1 + c->pk422 : c->dst32 ? 4 + (c->dst32 - FMT_ARGB) : c->dstFormat == FMT_BGR24 ? 1 : 0;
+    const PixFmt *D = c->D;
+    v.rangeConv = c->rangeConv; v.srcBits = c->srcFmt->bits;
+    v.k = c->k; v.flags = c->g.flags; v.planar = is_planar(D); v.dstBits = D->bits; v.dstBE = D->be; v.dstNV = D->fam == FAM_NV ? 1 + (D->fmt == PIX_NV21) : 0;
+    if (D->rgb16 || D->rgb48 || c->dstFmt->fam == FAM_GRAY || c->srcFmt->fam == FAM_GRAY) return false; // (the per-line slots do not cover the 15 / 16 / 12 / 48-bpp output stages: the hook leaves the C slots)
+    v.target = D->slot;
     return true;
 }
 
@@ -2177,8 +2201,8 @@ int sws_setColorspaceDetails_cuda(SwsContextCUDA *ctx, const int inv_table[4], i
     SwsCudaContext *c = (SwsCudaContext *)ctx;
     (void)table; (void)dstRange;                  // only read by the yuv -> yuv range conversion (not taken over) and rgb sources' fixed readers
     if (!c || !inv_table) { set_error_msg("sws_setColorspaceDetails_cuda", "NULL argument"); return -1; }
-    if (c->planar || c->pk422) return -1;         // isYUV(dstFormat): the reference returns -1 as well (utils.c:821-822)
-    if (c->special) return 0;                     // rgb -> rgb copies / swaps never look at the tables
+    if (is_planar(c->D) || c->D->pk422) return -1;         // isYUV(dstFormat): the reference returns -1 as well (utils.c:821-822)
+    if (!ROUTES[c->route].tables) return 0;       // rgb -> rgb copies / swaps never look at the tables
     RgbConstants k;
     rgb_constants(k, inv_table, srcRange != 0, brightness, contrast, saturation);
     if (k.cy <= 0) { set_error_msg("sws_setColorspaceDetails_cuda", "contrast must be positive"); return -1; }
@@ -2200,26 +2224,31 @@ int sws_scale_frames_cuda(SwsContextCUDA *ctx, const uint8_t *const src[3], cons
     SwsCudaContext *c = (SwsCudaContext *)ctx;
     if (!c) { set_error_msg("sws_scale_frames_cuda", "NULL context"); return -1; }
     static const size_t zero3[3] = { 0, 0, 0 };
-    if (c->srcGray && src && src[0] && srcStride && (!src[1] || !src[2])) {          // one plane: the luma plane stands in for the two nobody reads
-        const uint8_t *const s3[3] = { src[0], src[0], src[0] };
-        const int ss3[3] = { srcStride[0], srcStride[0], srcStride[0] };
-        const size_t sf3[3] = { srcFrameStride ? srcFrameStride[0] : 0, srcFrameStride ? srcFrameStride[0] : 0, srcFrameStride ? srcFrameStride[0] : 0 };
-        return sws_scale_frames_cuda(ctx, s3, ss3, sf3, dst, dstStride, dstFrameStride, nframes, stream);
+    const size_t *srcFrame = srcFrameStride ? srcFrameStride : zero3, *dstFrame = dstFrameStride ? dstFrameStride : zero3;
+    const uint8_t *s3[3]; int ss3[3]; size_t sf3[3];
+    if (c->srcFmt->fam == FAM_GRAY && src && src[0] && srcStride && (!src[1] || !src[2])) {     // one plane: the luma plane stands in for the two nobody reads
+        for (int p = 0; p < 3; p++) { s3[p] = src[0]; ss3[p] = srcStride[0]; sf3[p] = srcFrame[0]; }
+        src = s3; srcStride = ss3; srcFrame = sf3;
     }
-    if (c->gray && dst && dst[0] && dstStride) {      // chroma to scratch (every frame of the batch into the same two planes: nobody reads them)
-        uint8_t *const d3[3] = { dst[0], c->d_gray[0], c->d_gray[1] };
-        const int ds3[3] = { dstStride[0], c->grayPitch, c->grayPitch };
-        const size_t df3[3] = { dstFrameStride ? dstFrameStride[0] : 0, 0, 0 };
-        if (!src || !src[0] || (!c->srcPacked && (!src[1] || (!c->srcNV && !src[2])))) { set_error_msg("sws_scale_frames_cuda", "bad image pointers"); return -1; }
-        if (run_frames(c, src, srcStride, srcFrameStride ? srcFrameStride : zero3, d3, ds3, df3, nframes, (cudaStream_t)stream)) return -1;
-        return c->g.dstH * nframes;
+    uint8_t *d3[3]; int ds3[3]; size_t df3[3];
+    if (c->dstFmt->fam == FAM_GRAY && dst && dst[0] && dstStride) {       // chroma to scratch (every frame of the batch into the same two planes: nobody reads them)
+        d3[0] = dst[0]; d3[1] = c->d_gray[0]; d3[2] = c->d_gray[1];
+        ds3[0] = dstStride[0]; ds3[1] = ds3[2] = c->grayPitch;
+        df3[0] = dstFrame[0]; df3[1] = df3[2] = 0;
+        dst = d3; dstStride = ds3; dstFrame = df3;
+    } else if (c->S->fam == FAM_PAL8 && src && !src[1]) {
+        set_error_msg("sws_scale_frames_cuda", "a pal8 batch needs its palettes in plane 1 (device pointer, 1024 bytes per frame)"); return -1;
     }
-    if (c->srcPacked == 5 && src && !src[1]) { set_error_msg("sws_scale_frames_cuda", "a pal8 batch needs its palettes in plane 1 (device pointer, 1024 bytes per frame)"); return -1; }
-    if (!src || !dst || !src[0] || (!c->srcPacked && (!src[1] || (!c->srcNV && !src[2]))) || !dst[0] || (c->planar && (!dst[1] || (!c->dstNV && !dst[2])))) { set_error_msg("sws_scale_frames_cuda", "bad image pointers"); return -1; }
-    if (run_frames(c, src, srcStride, srcFrameStride ? srcFrameStride : zero3, dst, dstStride, dstFrameStride ? dstFrameStride : zero3,
-                   nframes, (cudaStream_t)stream)) return -1;
+    const bool pk = is_packed_src(c->S), nv = c->S->fam == FAM_NV;
+    if (!src || !dst || !src[0] || (!pk && (!src[1] || (!nv && !src[2]))) || !dst[0] || (is_planar(c->D) && (!dst[1] || (c->D->fam != FAM_NV && !dst[2])))) {
+        set_error_msg("sws_scale_frames_cuda", "bad image pointers"); return -1;
+    }
+    if (run_frames(c, src, srcStride, srcFrame, dst, dstStride, dstFrame, nframes, (cudaStream_t)stream)) return -1;
     return c->g.dstH * nframes;
 }
+
+static int scale_host(SwsCudaContext *c, const uint8_t *const srcSlice[], const int srcStride[], int srcSliceY, int srcSliceH,
+                      uint8_t *const dst[], const int dstStride[]);
 
 // Bottom-up pictures (negative strides, e.g. after a vertical flip that only negates linesize; the reference handles them like any
 // other stride, swscale_unscaled.c:1212-1340): the planes with a negative stride are copied row by row into top-down host buffers of the
@@ -2228,42 +2257,35 @@ int sws_scale_frames_cuda(SwsContextCUDA *ctx, const uint8_t *const src[3], cons
 // top-down path may look at or write (odd widths, pair rounding) -- never more than the pitch.
 static int sws_scale_cuda_flipped(SwsCudaContext *c, const uint8_t *const srcSlice[], const int srcStride[], int srcSliceH, uint8_t *const dst[], const int dstStride[])
 {
-    const SwsGeometry &g = c->g;
-    const bool pk = c->srcPacked != 0, nv = c->srcNV != 0, rgb = !c->planar;
-    const int pkBpp = c->srcPacked == 1 ? 3 : c->srcPacked == 4 ? 4 : c->srcPacked == 5 ? 1 : 2, sB = c->dstBits > 8 ? 2 : 1, pxB = c->rgb48 ? 6 : (c->pk422 || c->rgb16) ? 2 : c->dst32 ? 4 : 3;
-    const int nsrc = pk ? 1 : nv ? 2 : 3, ndst = rgb ? 1 : c->dstNV ? 2 : 3;
-    const int srcRows[3] = { g.srcH, g.chrSrcH, g.chrSrcH }, dstRows[3] = { g.dstH, g.chrDstH, g.chrDstH };
-    const size_t sS = c->srcBits > 8 ? 2 : 1;
-    const size_t srcW[3] = { (size_t)g.srcW * (pk ? pkBpp : sS), (size_t)g.chrSrcW * (nv ? 2 : sS), (size_t)g.chrSrcW * sS };
-    const size_t dstW[3] = { (size_t)g.dstW * (rgb ? pxB : sB), (size_t)g.chrDstW * (c->dstNV ? 2 : sB), (size_t)g.chrDstW * sB };
+    const PlaneGeom S = src_planes(c), D = dst_planes(c);
     std::vector<uint8_t> sbuf[3], dbuf[3];
     const uint8_t *s2[4] = { nullptr, nullptr, nullptr, nullptr };
     uint8_t *d2[4] = { nullptr, nullptr, nullptr, nullptr };
     int ss[4] = { 0, 0, 0, 0 }, ds[4] = { 0, 0, 0, 0 };
     size_t drow[3] = { 0, 0, 0 };
-    if (c->srcPacked == 5) { s2[1] = srcSlice[1]; ss[1] = srcStride[1]; }       // (pal8: the palette travels as it is)
-    for (int p = 0; p < nsrc; p++) {
+    if (c->S->fam == FAM_PAL8) { s2[1] = srcSlice[1]; ss[1] = srcStride[1]; }       // (pal8: the palette travels as it is)
+    for (int p = 0; p < S.n; p++) {
         s2[p] = srcSlice[p]; ss[p] = srcStride[p];
         if (srcStride[p] >= 0) continue;
-        const size_t pitch = (size_t)(-(ptrdiff_t)srcStride[p]), row = std::min(pitch, srcW[p] + 16);
-        sbuf[p].assign(pitch * srcRows[p] + 16, 0);
-        for (int y = 0; y < srcRows[p]; y++) memcpy(sbuf[p].data() + y * pitch, srcSlice[p] + (ptrdiff_t)y * srcStride[p], row);
+        const size_t pitch = (size_t)(-(ptrdiff_t)srcStride[p]), row = std::min(pitch, S.row[p] + 16);
+        sbuf[p].assign(pitch * S.rows[p] + 16, 0);
+        for (int y = 0; y < S.rows[p]; y++) memcpy(sbuf[p].data() + y * pitch, srcSlice[p] + (ptrdiff_t)y * srcStride[p], row);
         s2[p] = sbuf[p].data(); ss[p] = (int)pitch;
     }
-    for (int p = 0; p < ndst; p++) {
+    for (int p = 0; p < D.n; p++) {
         d2[p] = dst[p]; ds[p] = dstStride[p];
         if (dstStride[p] >= 0) continue;
         const size_t pitch = (size_t)(-(ptrdiff_t)dstStride[p]);
-        drow[p] = std::min(pitch, dstW[p] + 16);
-        dbuf[p].assign(pitch * dstRows[p] + 16, 0);
-        for (int y = 0; y < dstRows[p]; y++) memcpy(dbuf[p].data() + y * pitch, dst[p] + (ptrdiff_t)y * dstStride[p], drow[p]);
+        drow[p] = std::min(pitch, D.row[p] + 16);
+        dbuf[p].assign(pitch * D.rows[p] + 16, 0);
+        for (int y = 0; y < D.rows[p]; y++) memcpy(dbuf[p].data() + y * pitch, dst[p] + (ptrdiff_t)y * dstStride[p], drow[p]);
         d2[p] = dbuf[p].data(); ds[p] = (int)pitch;
     }
-    const int r = sws_scale_cuda((SwsContextCUDA *)c, s2, ss, 0, srcSliceH, d2, ds);
+    const int r = scale_host(c, s2, ss, 0, srcSliceH, d2, ds);
     if (r <= 0) return r;
-    for (int p = 0; p < ndst; p++)
+    for (int p = 0; p < D.n; p++)
         if (dstStride[p] < 0)
-            for (int y = 0; y < dstRows[p]; y++) memcpy(dst[p] + (ptrdiff_t)y * dstStride[p], dbuf[p].data() + (size_t)y * ds[p], drow[p]);
+            for (int y = 0; y < D.rows[p]; y++) memcpy(dst[p] + (ptrdiff_t)y * dstStride[p], dbuf[p].data() + (size_t)y * ds[p], drow[p]);
     return r;
 }
 
@@ -2277,48 +2299,40 @@ static int sws_scale_cuda_sliced(SwsCudaContext *c, const uint8_t *const srcSlic
                                  uint8_t *const dst[], const int dstStride[])
 {
     const SwsGeometry &g = c->g;
-    const bool pk = c->srcPacked != 0, nv = c->srcNV != 0, rgb = !c->planar;
-    const int nsrc = pk ? 1 : nv ? 2 : 3, ndst = rgb ? 1 : c->dstNV ? 2 : 3;
+    const PlaneGeom S = src_planes(c), D = dst_planes(c);
+    const RouteFacts &rf = ROUTES[c->route];
     if (srcSliceY < 0 || srcSliceH < 0 || srcSliceY + srcSliceH > g.srcH) { set_error_msg("sws_scale_cuda", "slice outside the picture"); return 0; }
-    for (int p = 0; p < nsrc; p++) if (srcStride[p] < 0) { set_error_msg("sws_scale_cuda", "slices of bottom-up pictures are not taken over"); return 0; }
-    for (int p = 0; p < ndst; p++) if (dstStride[p] < 0) { set_error_msg("sws_scale_cuda", "slices of bottom-up pictures are not taken over"); return 0; }
+    for (int p = 0; p < S.n; p++) if (srcStride[p] < 0) { set_error_msg("sws_scale_cuda", "slices of bottom-up pictures are not taken over"); return 0; }
+    for (int p = 0; p < D.n; p++) if (dstStride[p] < 0) { set_error_msg("sws_scale_cuda", "slices of bottom-up pictures are not taken over"); return 0; }
     if (srcSliceY == 0) { c->sliceNextY = 0; c->sliceDstY = 0; }
     else if (srcSliceY != c->sliceNextY) {
         // (the reference also takes bottom-up slice orders, and answers "Slices start in the middle!" to a first slice that touches neither end)
         set_error_msg("sws_scale_cuda", "slices are taken over top-down and contiguous only"); return 0;
     }
     const int end = srcSliceY + srcSliceH;
-    const bool rowMapped = c->copy || c->table_unscaled || c->special || c->to422 || c->nvcopy;
     {
         // a slice boundary inside a source chroma row makes the reference's scaler loop address rows before the slice (it has no check for it);
         // the unscaled converters work on whole chroma row groups of either side
-        int sub = g.chrSrcVSub;
-        if (rowMapped) {
-            sub = sub > g.chrDstVSub ? sub : g.chrDstVSub;
-            if (c->table_unscaled || c->special == 3 || c->to422 == 2) sub = sub > 1 ? sub : 1;
-        }
+        const int sub = rf.rowMapped ? std::max({ g.chrSrcVSub, g.chrDstVSub, rf.chrAlign }) : g.chrSrcVSub;
         const int m = (1 << sub) - 1;
         if ((srcSliceY & m) || ((srcSliceH & m) && end != g.srcH)) { set_error_msg("sws_scale_cuda", "slice not aligned to the chroma rows"); return 0; }
     }
     // keep the rows
-    const int sS = c->srcBits > 8 ? 2 : 1, pkBpp = c->srcPacked == 1 ? 3 : c->srcPacked == 4 ? 4 : c->srcPacked == 5 ? 1 : 2;
-    const int srcRows[3] = { g.srcH, g.chrSrcH, g.chrSrcH };
-    const size_t srcWB[3] = { (size_t)g.srcW * (pk ? pkBpp : sS), (size_t)g.chrSrcW * (nv ? 2 : 1) * sS, (size_t)g.chrSrcW * sS };
     const int cY0 = srcSliceY >> g.chrSrcVSub, cY1 = -((-end) >> g.chrSrcVSub);
-    for (int p = 0; p < nsrc; p++) {
+    for (int p = 0; p < S.n; p++) {
         const size_t pitch = (size_t)srcStride[p];
-        if (c->sliceSrc[p].size() != pitch * srcRows[p] + 16 || c->slicePitch[p] != srcStride[p]) {
+        if (c->sliceSrc[p].size() != pitch * S.rows[p] + 16 || c->slicePitch[p] != srcStride[p]) {
             if (srcSliceY != 0) { set_error_msg("sws_scale_cuda", "the source pitch changed between slices"); return 0; }
-            c->sliceSrc[p].assign(pitch * srcRows[p] + 16, 0);
+            c->sliceSrc[p].assign(pitch * S.rows[p] + 16, 0);
             c->slicePitch[p] = srcStride[p];
         }
-        const int y0 = p ? cY0 : srcSliceY, y1 = p ? (cY1 < srcRows[p] ? cY1 : srcRows[p]) : end;
-        const size_t row = pitch < srcWB[p] + 16 ? pitch : srcWB[p] + 16;
+        const int y0 = p ? cY0 : srcSliceY, y1 = p ? (cY1 < S.rows[p] ? cY1 : S.rows[p]) : end;
+        const size_t row = pitch < S.row[p] + 16 ? pitch : S.row[p] + 16;
         for (int y = y0; y < y1; y++) memcpy(c->sliceSrc[p].data() + (size_t)y * pitch, srcSlice[p] + (size_t)(y - y0) * pitch, row);
     }
     // the output rows this slice completes
     int dstY0, dstY1;
-    if (rowMapped) { dstY0 = srcSliceY; dstY1 = end; }
+    if (rf.rowMapped) { dstY0 = srcSliceY; dstY1 = end; }
     else {
         const int cdv = g.chrDstVSub, vL = c->vLum.size, vC = c->vChr.size;
         dstY0 = c->sliceDstY;
@@ -2331,34 +2345,31 @@ static int sws_scale_cuda_sliced(SwsCudaContext *c, const uint8_t *const srcSlic
     }
     c->sliceNextY = end == g.srcH ? 0 : end;
     c->sliceDstY = end == g.srcH ? 0 : dstY1;
-    const int ret = rowMapped ? srcSliceH : dstY1 - dstY0;
+    const int ret = rf.rowMapped ? srcSliceH : dstY1 - dstY0;
     if (dstY1 <= dstY0) return ret;
     // the frame pipeline over the rows so far, into a copy of the caller's picture; the finished rows go back
-    const int sB = c->dstBits > 8 ? 2 : 1, pxB = c->rgb48 ? 6 : (c->pk422 || c->rgb16) ? 2 : c->dst32 ? 4 : 3;
-    const int dstRows[3] = { g.dstH, g.chrDstH, g.chrDstH };
-    const size_t dstWB[3] = { (size_t)g.dstW * (rgb ? pxB : sB), (size_t)g.chrDstW * (c->dstNV ? 2 : sB), (size_t)g.chrDstW * sB };
     std::vector<uint8_t> dbuf[3];
     const uint8_t *s2[4] = { nullptr, nullptr, nullptr, nullptr };
     uint8_t *d2[4] = { nullptr, nullptr, nullptr, nullptr };
     int ss[4] = { 0, 0, 0, 0 }, ds[4] = { 0, 0, 0, 0 };
     size_t drow[3] = { 0, 0, 0 };
-    for (int p = 0; p < nsrc; p++) { s2[p] = c->sliceSrc[p].data(); ss[p] = srcStride[p]; }
-    if (c->srcPacked == 5) { s2[1] = srcSlice[1]; ss[1] = srcStride[1]; }         // (pal8: this slice's palette, like sws_scale() rebuilds its tables per call)
-    for (int p = 0; p < ndst; p++) {
+    for (int p = 0; p < S.n; p++) { s2[p] = c->sliceSrc[p].data(); ss[p] = srcStride[p]; }
+    if (c->S->fam == FAM_PAL8) { s2[1] = srcSlice[1]; ss[1] = srcStride[1]; }         // (pal8: this slice's palette, like sws_scale() rebuilds its tables per call)
+    for (int p = 0; p < D.n; p++) {
         const size_t pitch = (size_t)dstStride[p];
-        drow[p] = pitch < dstWB[p] + 16 ? pitch : dstWB[p] + 16;
-        dbuf[p].assign(pitch * dstRows[p] + 16, 0);
-        for (int y = 0; y < dstRows[p]; y++) memcpy(dbuf[p].data() + (size_t)y * pitch, dst[p] + (size_t)y * pitch, drow[p]);
+        drow[p] = pitch < D.row[p] + 16 ? pitch : D.row[p] + 16;
+        dbuf[p].assign(pitch * D.rows[p] + 16, 0);
+        for (int y = 0; y < D.rows[p]; y++) memcpy(dbuf[p].data() + (size_t)y * pitch, dst[p] + (size_t)y * pitch, drow[p]);
         d2[p] = dbuf[p].data(); ds[p] = dstStride[p];
     }
-    if (sws_scale_cuda((SwsContextCUDA *)c, s2, ss, 0, g.srcH, d2, ds) <= 0) return 0;
+    if (scale_host(c, s2, ss, 0, g.srcH, d2, ds) <= 0) return 0;
     c->sliceNextY = end == g.srcH ? 0 : end;          // (the whole-frame call above restarted the slice state)
     c->sliceDstY = end == g.srcH ? 0 : dstY1;
     const int s = 1 << g.chrDstVSub;
-    for (int p = 0; p < ndst; p++) {
+    for (int p = 0; p < D.n; p++) {
         const int y0 = p ? (dstY0 + s - 1) >> g.chrDstVSub : dstY0;
         int y1 = p ? (dstY1 + s - 1) >> g.chrDstVSub : dstY1;
-        if (y1 > dstRows[p]) y1 = dstRows[p];
+        if (y1 > D.rows[p]) y1 = D.rows[p];
         for (int y = y0; y < y1; y++) memcpy(dst[p] + (size_t)y * ds[p], dbuf[p].data() + (size_t)y * ds[p], drow[p]);
     }
     return ret;
@@ -2372,40 +2383,50 @@ int sws_scale_cuda(SwsContextCUDA *ctx, const uint8_t *const srcSlice[], const i
     avb::enter();
     SwsCudaContext *c = (SwsCudaContext *)ctx;
     if (!c || srcSliceH == 0) return 0;
-    if (c->srcGray && srcSlice && srcSlice[0] && srcStride && (!srcSlice[1] || !srcSlice[2] || srcStride[1] != srcStride[0] || srcStride[2] != srcStride[0])) {
+    const uint8_t *s4[4]; int ss4[4];
+    if (c->srcFmt->fam == FAM_GRAY && srcSlice && srcSlice[0] && srcStride && (!srcSlice[1] || !srcSlice[2] || srcStride[1] != srcStride[0] || srcStride[2] != srcStride[0])) {
         // a gray8 picture has one plane (data[1] of an AVFrame is its pseudo-palette): the luma plane stands in for the two planes nobody reads
-        const uint8_t *const s4[4] = { srcSlice[0], srcSlice[0], srcSlice[0], nullptr };
-        const int ss4[4] = { srcStride[0], srcStride[0], srcStride[0], 0 };
-        return sws_scale_cuda(ctx, s4, ss4, srcSliceY, srcSliceH, dst, dstStride);
+        for (int p = 0; p < 3; p++) { s4[p] = srcSlice[0]; ss4[p] = srcStride[0]; }
+        s4[3] = nullptr; ss4[3] = 0;
+        srcSlice = s4; srcStride = ss4;
     }
-    if (c->gray && dst && dst[0] && dstStride) {        // (a gray8 caller's dst[] has one plane; `gray` is cleared around the inner call)
+    uint8_t *d4[4]; int ds4[4];
+    if (c->dstFmt->fam == FAM_GRAY && dst && dst[0] && dstStride) {        // (a gray8 caller's dst[] has one plane)
         if (srcSliceY != 0 || srcSliceH != c->g.srcH) {
             // the rows a slice completes follow the destination's chroma geometry; a gray8 destination has none in the reference (chrDstVSubSample 0,
             // its own vertical chroma filter) while this context carries the planar stand-in's: whole frames only
             set_error_msg("sws_scale_cuda", "slices into a gray8 destination are not taken over (whole frames are)"); return 0;
         }
-        // the chroma planes of the planar conversion go to host scratch of the context (they are computed and dropped)
+        // the chroma planes of the planar conversion go to host scratch of the context (they are computed and dropped); bottom-up: the scratch
+        // planes are addressed from their last row like the caller's plane
         const size_t bytes = (size_t)c->grayPitch * (c->g.chrDstH + 2);
-        for (int k = 0; k < 2; k++) if (c->h_gray[k].size() < bytes) c->h_gray[k].resize(bytes);
-        uint8_t *const d3[4] = { dst[0], c->h_gray[0].data(), c->h_gray[1].data(), nullptr };
-        const int ds3[4] = { dstStride[0], dstStride[0] < 0 ? -c->grayPitch : c->grayPitch, dstStride[0] < 0 ? -c->grayPitch : c->grayPitch, 0 };
-        if (dstStride[0] < 0) {              // bottom-up: the scratch planes are addressed from their last row like the caller's plane
-            uint8_t *const d3f[4] = { dst[0], c->h_gray[0].data() + (size_t)c->grayPitch * (c->g.chrDstH - 1), c->h_gray[1].data() + (size_t)c->grayPitch * (c->g.chrDstH - 1), nullptr };
-            c->gray = false; const int r = sws_scale_cuda(ctx, srcSlice, srcStride, srcSliceY, srcSliceH, d3f, ds3); c->gray = true; return r;
+        const bool up = dstStride[0] < 0;
+        for (int k = 0; k < 2; k++) {
+            if (c->h_gray[k].size() < bytes) c->h_gray[k].resize(bytes);
+            d4[1 + k] = c->h_gray[k].data() + (up ? (size_t)c->grayPitch * (c->g.chrDstH - 1) : 0);
+            ds4[1 + k] = up ? -c->grayPitch : c->grayPitch;
         }
-        c->gray = false; const int r = sws_scale_cuda(ctx, srcSlice, srcStride, srcSliceY, srcSliceH, d3, ds3); c->gray = true; return r;
+        d4[0] = dst[0]; ds4[0] = dstStride[0]; d4[3] = nullptr; ds4[3] = 0;
+        dst = d4; dstStride = ds4;
     }
-    const bool rgb = !c->planar;
-    const bool nv = c->srcNV != 0, pk = c->srcPacked != 0;
+    return scale_host(c, srcSlice, srcStride, srcSliceY, srcSliceH, dst, dstStride);
+}
+
+// sws_scale_cuda on the planes as given
+static int scale_host(SwsCudaContext *c, const uint8_t *const srcSlice[], const int srcStride[], int srcSliceY, int srcSliceH,
+                      uint8_t *const dst[], const int dstStride[])
+{
+    const bool rgb = !is_planar(c->D);
+    const bool nv = c->S->fam == FAM_NV, pk = is_packed_src(c->S), dstNV = c->D->fam == FAM_NV;
     if (!srcSlice || !dst || !srcSlice[0] || !srcStride[0] || (!pk && (!srcSlice[1] || !srcStride[1] || (!nv && (!srcSlice[2] || !srcStride[2])))) ||
-        !dst[0] || !dstStride[0] || (!rgb && (!dst[1] || !dstStride[1] || (!c->dstNV && (!dst[2] || !dstStride[2]))))) {
+        !dst[0] || !dstStride[0] || (!rgb && (!dst[1] || !dstStride[1] || (!dstNV && (!dst[2] || !dstStride[2]))))) {
         set_error_msg("sws_scale_cuda", "bad image pointers"); return 0;
     }
-    if (c->srcPacked == 5 && !srcSlice[1]) { set_error_msg("sws_scale_cuda", "a pal8 picture needs its palette in plane 1"); return 0; }
+    if (c->S->fam == FAM_PAL8 && !srcSlice[1]) { set_error_msg("sws_scale_cuda", "a pal8 picture needs its palette in plane 1"); return 0; }
     if (srcSliceY != 0 || srcSliceH != c->g.srcH) return sws_scale_cuda_sliced(c, srcSlice, srcStride, srcSliceY, srcSliceH, dst, dstStride);
     c->sliceNextY = 0; c->sliceDstY = 0;
     if (srcStride[0] < 0 || (!pk && (srcStride[1] < 0 || (!nv && srcStride[2] < 0))) || dstStride[0] < 0 ||
-        (!rgb && (dstStride[1] < 0 || (!c->dstNV && dstStride[2] < 0))))
+        (!rgb && (dstStride[1] < 0 || (!dstNV && dstStride[2] < 0))))
         return sws_scale_cuda_flipped(c, srcSlice, srcStride, srcSliceH, dst, dstStride);
     // the context's own three streams: like the reference's SwsContext a context serves one thread at a time (swscale.c:393-398), and
     // contexts of different threads run concurrently -- eight streams keep both PCIe directions busy where one leaves bubbles between
@@ -2418,30 +2439,26 @@ int sws_scale_cuda(SwsContextCUDA *ctx, const uint8_t *const srcSlice[], const i
     cudaStream_t *st = c->streams;
     cudaStream_t s = st[0];
     const SwsGeometry &g = c->g;
-    // device staging: tight, aligned pitches
-    // (a packed source keeps the caller's pitch: the chroma readers look one pixel past an odd width, into the padding or the next row)
-    const int pkBpp = c->srcPacked == 1 ? 3 : c->srcPacked == 4 ? 4 : c->srcPacked == 5 ? 1 : 2;
-    const int sS = c->srcBits > 8 ? 2 : 1;                  // bytes per source sample (planar 9 / 10 / 16-bit sources)
-    const int yP = pk ? srcStride[0] : (g.srcW * sS + 15) & ~15, cP = ((nv ? 2 : 1) * g.chrSrcW * sS + 15) & ~15;
-    const size_t yB = (size_t)yP * g.srcH, cB = pk ? 0 : (size_t)cP * g.chrSrcH;
-    const size_t needS = yB + (nv ? 1 : 2) * cB;
+    // device staging: tight, aligned pitches (a packed source keeps the caller's pitch: the chroma readers look one pixel past an odd
+    // width, into the padding or the next row; a packed destination gets room for the pixel past an odd width)
+    const PlaneGeom SP = src_planes(c), DP = dst_planes(c);
     const int odd = g.dstW & 1;
-    const int sB = c->dstBits > 8 ? 2 : 1;                  // bytes per sample of a planar destination
-    const int pxB = c->rgb48 ? 6 : (c->pk422 || c->rgb16) ? 2 : c->dst32 ? 4 : 3;        // bytes per packed pixel
-    const int dP = rgb ? ((g.dstW + odd) * pxB + 15) & ~15 : (g.dstW * sB + 15) & ~15, dcP = (g.chrDstW * sB * (c->dstNV ? 2 : 1) + 15) & ~15;
-    const size_t dB = (size_t)dP * g.dstH, dcB = rgb ? 0 : (size_t)dcP * g.chrDstH;
-    const size_t needD = dB + 2 * dcB;
-    if (c->src_bytes < needS) { cudaFree(c->d_src); c->d_src = nullptr; if (cudaMalloc(&c->d_src, needS) != cudaSuccess) { set_error("sws_scale_cuda", cudaGetLastError()); return 0; } c->src_bytes = needS; }
-    if (c->dst_bytes < needD) { cudaFree(c->d_dst); c->d_dst = nullptr; if (cudaMalloc(&c->d_dst, needD) != cudaSuccess) { set_error("sws_scale_cuda", cudaGetLastError()); return 0; } c->dst_bytes = needD; }
-    const uint8_t *ds[3] = { c->d_src, c->srcPacked == 5 ? c->d_pal : c->d_src + yB, c->d_src + yB + cB };     // (pal8: plane 1 is the palette)
-    uint8_t *dd[3] = { c->d_dst, c->d_dst + dB, c->d_dst + dB + dcB };
-    const int dsS[3] = { yP, cP, cP }, ddS[3] = { dP, dcP, dcP };
+    int sP[3], dP[3];
+    size_t sOff[4] = { 0 }, dOff[4] = { 0 };
+    for (int p = 0; p < 3; p++) {
+        sP[p] = pk && !p ? srcStride[0] : (int)((SP.row[p] + 15) & ~(size_t)15);
+        dP[p] = (int)((DP.row[p] + (rgb && odd ? c->D->bpp : 0) + 15) & ~(size_t)15);
+        sOff[p + 1] = sOff[p] + (p < SP.n ? (size_t)sP[p] * SP.rows[p] : 0);
+        dOff[p + 1] = dOff[p] + (p < DP.n ? (size_t)dP[p] * DP.rows[p] : 0);
+    }
+    if (grow(c->d_src, c->src_bytes, sOff[3], s, "sws_scale_cuda") || grow(c->d_dst, c->dst_bytes, dOff[3], s, "sws_scale_cuda")) return 0;
+    const uint8_t *ds[3] = { c->d_src, c->S->fam == FAM_PAL8 ? c->d_pal : c->d_src + sOff[1], c->d_src + sOff[2] };     // (pal8: plane 1 is the palette)
+    uint8_t *dd[3] = { c->d_dst, c->d_dst + dOff[1], c->d_dst + dOff[2] };
     // Same-size rgb (the dp4a fused kernel): the frame goes through in bands of rows on three streams, so the upload of band
     // k + 1, the kernel of band k and the download of band k - 1 overlap -- the call is PCIe bound and PCIe is full duplex.
     // A band re-uploads the few chroma lines it shares with its neighbours (identical bytes), so bands need no cross-stream order.
-    if (c->fused && c->fast_ok && !nv && rgb && !c->dst32 && !odd && tuning("sws_fused_variant") != 1 &&
+    if (c->route == R_FUSED && c->fast_ok && !nv && c->D->fam == FAM_RGB24 && !odd && tuning("sws_fused_variant") != 1 &&
         tuning("sws_host_bands") != 1 && g.dstH >= 64 && !((uintptr_t)c->dev.vChrF & 15)) {
-        const SwsDev &p = c->dev;
         const int pairs = g.dstH / 2, nb = tuning("sws_host_bands") > 1 ? tuning("sws_host_bands") : 3, per = ((pairs + nb - 1) / nb + 3) & ~3;
         int k = 0;
         for (int rp0 = 0; rp0 < pairs; rp0 += per, k = (k + 1) % 3) {
@@ -2449,77 +2466,62 @@ int sws_scale_cuda(SwsContextCUDA *ctx, const uint8_t *const srcSlice[], const i
             cudaStream_t sb = st[k];
             int clo = c->vChr.pos[y0] > -3 ? c->vChr.pos[y0] : -3, chi = (c->vChr.pos[y1 - 1] > -3 ? c->vChr.pos[y1 - 1] : -3) + 4;
             clo = clo < 0 ? 0 : clo; chi = chi > g.chrSrcH - 1 ? g.chrSrcH - 1 : chi;
-            if (cudaMemcpy2DAsync((void *)(ds[0] + (size_t)y0 * yP), yP, srcSlice[0] + (size_t)y0 * srcStride[0], srcStride[0], g.srcW, y1 - y0, cudaMemcpyHostToDevice, sb) != cudaSuccess ||
-                cudaMemcpy2DAsync((void *)(ds[1] + (size_t)clo * cP), cP, srcSlice[1] + (size_t)clo * srcStride[1], srcStride[1], g.chrSrcW, chi - clo + 1, cudaMemcpyHostToDevice, sb) != cudaSuccess ||
-                cudaMemcpy2DAsync((void *)(ds[2] + (size_t)clo * cP), cP, srcSlice[2] + (size_t)clo * srcStride[2], srcStride[2], g.chrSrcW, chi - clo + 1, cudaMemcpyHostToDevice, sb) != cudaSuccess) {
+            if (cudaMemcpy2DAsync((void *)(ds[0] + (size_t)y0 * sP[0]), sP[0], srcSlice[0] + (size_t)y0 * srcStride[0], srcStride[0], g.srcW, y1 - y0, cudaMemcpyHostToDevice, sb) != cudaSuccess ||
+                cudaMemcpy2DAsync((void *)(ds[1] + (size_t)clo * sP[1]), sP[1], srcSlice[1] + (size_t)clo * srcStride[1], srcStride[1], g.chrSrcW, chi - clo + 1, cudaMemcpyHostToDevice, sb) != cudaSuccess ||
+                cudaMemcpy2DAsync((void *)(ds[2] + (size_t)clo * sP[2]), sP[2], srcSlice[2] + (size_t)clo * srcStride[2], srcStride[2], g.chrSrcW, chi - clo + 1, cudaMemcpyHostToDevice, sb) != cudaSuccess) {
                 set_error("sws_scale_cuda:h2d", cudaGetLastError()); return 0;
             }
-            FusedArgs a;
-            a.y = ds[0]; a.u = ds[1]; a.v = ds[2]; a.dst = dd[0];
-            a.yStride = yP; a.uStride = cP; a.vStride = cP; a.dstStride = dP;
-            a.yFrame = a.uFrame = a.vFrame = a.dstFrame = 0;
+            static const size_t zero3[3] = { 0, 0, 0 };
+            FusedArgs a = fused_args(ds, sP, zero3, dd[0], dP[0], 0);
             a.rp0 = rp0; a.rp1 = rp1;
             if (launch_fused_fast(c, a, 1, sb)) return 0;
-            if (cudaMemcpy2DAsync(dst[0] + (size_t)y0 * dstStride[0], dstStride[0], dd[0] + (size_t)y0 * dP, dP, (size_t)g.dstW * 3, y1 - y0, cudaMemcpyDeviceToHost, sb) != cudaSuccess) {
+            if (cudaMemcpy2DAsync(dst[0] + (size_t)y0 * dstStride[0], dstStride[0], dd[0] + (size_t)y0 * dP[0], dP[0], (size_t)g.dstW * 3, y1 - y0, cudaMemcpyDeviceToHost, sb) != cudaSuccess) {
                 set_error("sws_scale_cuda:d2h", cudaGetLastError()); return 0;
             }
         }
         for (int q = 0; q < 3; q++) if (cudaStreamSynchronize(st[q]) != cudaSuccess) { set_error("sws_scale_cuda:sync", cudaGetLastError()); return 0; }
         return g.dstH;
     }
-    // planar -> packed 4:2:2 converters: the rounded-up last pair reads the samples just past the width (see run_frames_24)
+    // planar -> packed 4:2:2 converters: the rounded-up last pair reads the samples just past the width (to422_pairs)
     int upX = 0, upCX = 0;
-    if (c->to422 == 1 || c->to422 == 2) {
-        const int pairs = g.srcW >> 1, pairs_r = (pairs + 1) & ~1;
-        if (pairs_r > pairs && dstStride[0] >= 4 * pairs_r && srcStride[0] >= 2 * pairs_r && srcStride[1] >= pairs_r && srcStride[2] >= pairs_r) {
-            upX = 2 * pairs_r - g.srcW; upCX = pairs_r - g.chrSrcW;
-            if (upX < 0) upX = 0;
-            if (upCX < 0) upCX = 0;
-        }
+    if (c->route == R_422_FROM_422P || c->route == R_422_FROM_420P) {
+        const int np = to422_pairs(g.srcW, dstStride[0], srcStride);
+        upX = std::max(0, 2 * np - g.srcW); upCX = std::max(0, np - g.chrSrcW);
     }
     if (pk) {
-        size_t rowB = (size_t)g.srcW * pkBpp;
-        if ((g.srcW & 1) && rowB + pkBpp <= (size_t)srcStride[0]) rowB += pkBpp;       // the pixel the readers look at past an odd width
+        const int bpp = c->S->bpp;
+        size_t rowB = (size_t)g.srcW * bpp;
+        if ((g.srcW & 1) && rowB + bpp <= (size_t)srcStride[0]) rowB += bpp;       // the pixel the readers look at past an odd width
         if (cudaMemcpyAsync((void *)ds[0], srcSlice[0], (size_t)(g.srcH - 1) * srcStride[0] + rowB, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-            (c->srcPacked == 5 && cudaMemcpyAsync(c->d_pal, srcSlice[1], 1024, cudaMemcpyHostToDevice, s) != cudaSuccess)) {
+            (c->S->fam == FAM_PAL8 && cudaMemcpyAsync(c->d_pal, srcSlice[1], 1024, cudaMemcpyHostToDevice, s) != cudaSuccess)) {
             set_error("sws_scale_cuda:h2d", cudaGetLastError()); return 0;
         }
-    } else if (cudaMemcpy2DAsync((void *)ds[0], yP, srcSlice[0], srcStride[0], (size_t)(g.srcW + upX) * sS, g.srcH, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemcpy2DAsync((void *)ds[1], cP, srcSlice[1], srcStride[1], (size_t)((nv ? 2 : 1) * g.chrSrcW + upCX) * sS, g.chrSrcH, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        (!nv && cudaMemcpy2DAsync((void *)ds[2], cP, srcSlice[2], srcStride[2], (size_t)(g.chrSrcW + upCX) * sS, g.chrSrcH, cudaMemcpyHostToDevice, s) != cudaSuccess)) {
-        set_error("sws_scale_cuda:h2d", cudaGetLastError()); return 0;
+    } else {
+        const size_t sS = c->srcFmt->bits > 8 ? 2 : 1;
+        for (int p = 0; p < SP.n; p++)
+            if (cudaMemcpy2DAsync((void *)ds[p], sP[p], srcSlice[p], srcStride[p], SP.row[p] + (p ? upCX : upX) * sS, SP.rows[p], cudaMemcpyHostToDevice, s) != cudaSuccess) {
+                set_error("sws_scale_cuda:h2d", cudaGetLastError()); return 0;
+            }
     }
     static const size_t zero3[3] = { 0, 0, 0 };
-    if (run_frames(c, ds, dsS, zero3, dd, ddS, zero3, 1, s)) return 0;
+    if (run_frames(c, ds, sP, zero3, dd, dP, zero3, 1, s)) return 0;
     cudaError_t e;
     if (rgb) {
-        // whole pixel pairs are written (one pixel past an odd width) when the caller's stride has room
-        size_t wbytes = (size_t)g.dstW * pxB;
-        if (odd && !c->dev.full && (size_t)dstStride[0] >= wbytes + pxB) wbytes += pxB;      // (full chroma writes single pixels)
-        if (c->table_unscaled) wbytes = (size_t)(g.dstW & ~1) * pxB;       // that converter leaves an odd last column untouched
-        if (c->special) wbytes = (size_t)g.dstW * (c->dst32 ? 4 : 3);
-        if (c->to422) {          // (see run_frames_24: an odd pair count is rounded up when the rows have room)
-            const int pairs = g.dstW >> 1, pairs_r = (pairs + 1) & ~1;
-            const bool extra = pairs_r > pairs && dstStride[0] >= 4 * pairs_r && srcStride[0] >= 2 * pairs_r && srcStride[1] >= pairs_r && srcStride[2] >= pairs_r;
-            wbytes = c->to422 == 3 ? (size_t)g.dstW * 2 : (size_t)(extra ? pairs_r : pairs) * 4;
-        }
-        e = cudaMemcpy2DAsync(dst[0], dstStride[0], dd[0], dP, wbytes, g.dstH, cudaMemcpyDeviceToHost, s);
+        e = cudaMemcpy2DAsync(dst[0], dstStride[0], dd[0], dP[0], (size_t)packed_cols(c, dstStride[0], srcStride) * c->D->bpp, g.dstH, cudaMemcpyDeviceToHost, s);
     } else {
-        // rgb24toyv12_c converts whole pixel pairs only
-        e = cudaMemcpy2DAsync(dst[0], dstStride[0], dd[0], dP, (size_t)(c->special == 3 ? g.dstW & ~1 : g.dstW) * sB, g.dstH, cudaMemcpyDeviceToHost, s);
-        // nv12ToPlanarWrapper splits srcW / 2 x srcH / 2 samples: an odd last column / row of the caller's planes stays untouched;
-        // the packed -> yuv420p converters write srcH / 2 chroma rows
-        const int cw = ((nv && c->copy) || c->special == 3 || c->nvcopy) ? g.srcW / 2 : g.chrDstW;
-        const int ch = ((nv && c->copy) || (c->special >= 3 && c->special <= 5) || c->nvcopy) ? g.srcH / 2 : g.chrDstH;
-        if (e == cudaSuccess && cw && ch) e = cudaMemcpy2DAsync(dst[1], dstStride[1], dd[1], dcP, (size_t)cw * sB * (c->dstNV ? 2 : 1), ch, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && cw && ch && !c->dstNV) e = cudaMemcpy2DAsync(dst[2], dstStride[2], dd[2], dcP, (size_t)cw * sB, ch, cudaMemcpyDeviceToHost, s);
+        int w, cw, ch;
+        planar_extent(c, w, cw, ch);
+        const size_t sB = c->D->bits > 8 ? 2 : 1;
+        e = cudaMemcpy2DAsync(dst[0], dstStride[0], dd[0], dP[0], (size_t)w * sB, g.dstH, cudaMemcpyDeviceToHost, s);
+        for (int p = 1; p < DP.n && e == cudaSuccess && cw && ch; p++)
+            e = cudaMemcpy2DAsync(dst[p], dstStride[p], dd[p], dP[p], (size_t)cw * sB * (dstNV ? 2 : 1), ch, cudaMemcpyDeviceToHost, s);
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) { set_error("sws_scale_cuda:d2h", e); return 0; }
     return g.dstH;
 }
 
-int sws_is_fused_cuda(SwsContextCUDA *ctx) { avb::enter(); return ctx ? ((SwsCudaContext *)ctx)->fused : 0; }
+int sws_is_fused_cuda(SwsContextCUDA *ctx) { avb::enter(); return ctx ? ((SwsCudaContext *)ctx)->route == R_FUSED : 0; }
 
 // Host-only introspection used by the CPU test-suite to pin the set-up stage against the reference
 // (no device is touched): filter bank `which` (0 hLum, 1 hChr, 2 vLum, 3 vChr) of the context that
@@ -2537,7 +2539,7 @@ int sws_debug_filter2_cuda(int which, int srcW, int srcH, int dstW, int dstH, in
                            int16_t *filter, int32_t *pos, int cap, int *n_out)
 {
     avb::enter();
-    SwsCudaContext *c = make_context(srcW, srcH, FMT_YUV420P, dstW, dstH, dstFormat, flags, nullptr, false, srcFilter, dstFilter);
+    SwsCudaContext *c = make_context(srcW, srcH, PIX_YUV420P, dstW, dstH, dstFormat, flags, nullptr, false, srcFilter, dstFilter);
     if (!c) return -1;
     const FilterBank &b = which == 0 ? c->hLum : which == 1 ? c->hChr : which == 2 ? c->vLum : c->vChr;
     int fs = b.size;
@@ -2550,8 +2552,8 @@ int sws_debug_filter2_cuda(int which, int srcW, int srcH, int dstW, int dstH, in
 // What sws_getContext_cuda() decides for a request, without touching a device (CPU tests of the format / refusal rules):
 // returns 1 and fills out[] when the request is taken over, 0 (with the error string set) when it is refused.
 //   out[0] path: 1 plane copy (planarCopyWrapper / nv12ToPlanarWrapper), 2 unscaled table converter, 3 fused same-size kernel,
-//          4 general scaler (tile kernel or two passes), 5 packed-source special converter, 6 planar -> packed 4:2:2 converter,
-//          7 yuv420p -> nv12 / nv21 interleave
+//          4 general scaler (tile kernel or two passes) and the 48-bit rgb kernel, 5 the unscaled converters for packed sources, rgb pairs,
+//          gray8 and pal8 to rgb, 6 planar -> packed 4:2:2 converter, 7 yuv420p -> nv12 / nv21 interleave
 //   out[1..4] chrSrcW, chrSrcH, chrDstW, chrDstH   out[5] source pre-pass: 0 none, 1 nv split, 2 packed reader
 //   out[6] destination sample bits (planar) or bytes per pixel (packed)   out[7] full-range source
 int sws_debug_plan_cuda(int srcW, int srcH, int srcFormat, int dstW, int dstH, int dstFormat, int flags, int32_t out[8])
@@ -2559,10 +2561,10 @@ int sws_debug_plan_cuda(int srcW, int srcH, int srcFormat, int dstW, int dstH, i
     avb::enter();
     SwsCudaContext *c = make_context(srcW, srcH, srcFormat, dstW, dstH, dstFormat, flags, nullptr, false);
     if (!c) return 0;
-    out[0] = c->to422 ? 6 : c->nvcopy ? 7 : c->special ? 5 : c->copy ? 1 : c->table_unscaled ? 2 : c->fused ? 3 : 4;
+    out[0] = ROUTES[c->route].plan;
     out[1] = c->g.chrSrcW; out[2] = c->g.chrSrcH; out[3] = c->g.chrDstW; out[4] = c->g.chrDstH;
-    out[5] = c->srcPacked ? 2 : c->srcNV ? 1 : 0;
-    out[6] = c->planar ? c->dstBits : c->rgb48 ? 6 : (c->pk422 || c->rgb16) ? 2 : c->dst32 ? 4 : 3;
+    out[5] = is_packed_src(c->S) ? 2 : c->S->fam == FAM_NV ? 1 : 0;
+    out[6] = is_planar(c->D) ? c->D->bits : c->D->bpp;
     out[7] = c->srcRange;
     delete c;
     return 1;
