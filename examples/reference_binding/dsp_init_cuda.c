@@ -13,6 +13,7 @@
 #include "libavcodec/fdctdsp.h"
 #include "libavcodec/blockdsp.h"
 #include "libavcodec/me_cmp.h"
+#include "libavcodec/mpegvideodsp.h"
 #include "libavcodec/h263dsp.h"
 #include "libavcodec/h264dsp.h"
 #include "libavcodec/h264qpel.h"
@@ -40,6 +41,7 @@ void ff_hpeldsp_init_cuda(HpelDSPContext *c, int flags);
 void ff_pixblockdsp_init_cuda(PixblockDSPContext *c, unsigned high_bit_depth);
 void ff_qpeldsp_init_cuda(QpelDSPContext *c);
 void ff_h263dsp_init_cuda(H263DSPContext *c);
+void ff_mpegvideodsp_init_cuda(MpegVideoDSPContext *c);
 void ff_fft_init_cuda(FFTContext *s);
 void ff_mdct_init_cuda(FFTContext *s);
 
@@ -91,10 +93,12 @@ void ff_pixblockdsp_init_cuda_hook(PixblockDSPContext *c, AVCodecContext *avctx,
 /* the remaining tables take exactly the arguments of their x86 hooks: ff_blockdsp_init_cuda(c), ff_me_cmp_init_cuda(c),
  * ff_h264dsp_init_cuda(c, bit_depth, chroma_format_idc), ff_h264qpel_init_cuda(c, bit_depth), ff_h264chroma_init_cuda(c, bit_depth),
  * ff_h264_pred_init_cuda(h, codec_id, bit_depth, chroma_format_idc), ff_hpeldsp_init_cuda(c, flags), ff_qpeldsp_init_cuda(c),
- * ff_fft_init_cuda(s), ff_mdct_init_cuda(s), ff_h263dsp_init_cuda(c) (h263dsp.c:122-123, after ff_h263dsp_init_x86) */
+ * ff_fft_init_cuda(s), ff_mdct_init_cuda(s), ff_h263dsp_init_cuda(c) (h263dsp.c:122-123, after ff_h263dsp_init_x86),
+ * ff_mpegvideodsp_init_cuda(c) (mpegvideo.c:274, after ff_mpegvideodsp_init(&s->mdsp)) */
 void all_hooks_take_the_reference_types(IDCTDSPContext *a, FDCTDSPContext *b, BlockDSPContext *c, MECmpContext *d, H264DSPContext *e,
                                         H264QpelContext *f, H264ChromaContext *g, H264PredContext *h, HpelDSPContext *i,
-                                        PixblockDSPContext *j, QpelDSPContext *k, FFTContext *l, H263DSPContext *m, AVCodecContext *avctx)
+                                        PixblockDSPContext *j, QpelDSPContext *k, FFTContext *l, H263DSPContext *m, MpegVideoDSPContext *n,
+                                        AVCodecContext *avctx)
 {
     ff_idctdsp_init_cuda_hook(a, avctx, avctx->bits_per_raw_sample > 8);
     ff_xvid_idct_init_cuda_hook(a, avctx);
@@ -111,6 +115,7 @@ void all_hooks_take_the_reference_types(IDCTDSPContext *a, FDCTDSPContext *b, Bl
     ff_fft_init_cuda(l);
     ff_mdct_init_cuda(l);
     ff_h263dsp_init_cuda(m);
+    ff_mpegvideodsp_init_cuda(n);
 }
 
 /* ---- MECmpContext.quant_psnr / bit / rd (INTEGRATION.md section 2a): called from ff_mpv_encode_init() after the quantiser, the matrices and the

@@ -513,8 +513,15 @@ int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *recs, size_t n, uint8_t *dst, c
  *   FFMpvOBMCRecord: the four 8x8 luma blocks as put_obmc weighted sums of hpel_motion predictions (put_no_rnd under no_rounding), chroma
  *   through chroma_4mv_motion with the sum of the four own vectors -- also for a 16X16 macroblock.  Its records must be forward-only
  *   (mv_dir & 3 == 1); others count as rejected.  obmc is ignored in B pictures, as in the C code.
- * Refused: GMC / sprites, OBMC in a quarter-sample, MPEG-1 / 2 or obmc_recs-less P picture, H.261, WMV2 mspel, field pictures and field
- * MC in the H.263 family, 4:2:2 / 4:4:4, lowres.  A picture
+ * GMC: an MPEG-4 S-VOP (sprite set: out_format 2, a frame picture, not b_picture, obmc 0, real_sprite_warping_points 1..3 and
+ *   sprite_warping_accuracy 0..3) runs, for a 16X16 record with mcsel set, gmc1_motion (real_sprite_warping_points 1) or gmc_motion
+ *   (2, 3) (mpegvideo_motion.c:37-190) from the picture's sprite_offset / sprite_delta, with put for every direction the record names;
+ *   its mv is not read.  Every other record of an S-VOP (mcsel 0, 8X8 with mcsel ignored, as in the C code) runs as in a P picture.
+ *   The sprite fields must be those mpeg4_decode_sprite_trajectory (mpeg4videodec.c:168-385) leaves: the C arithmetic, which the kernel
+ *   follows, is only defined where gmc_motion's and ff_gmc_c's intermediates fit int32 (the kernel's affine map is that arithmetic
+ *   mod 2^32 all the same).
+ * Refused: static sprites and any other sprite picture, OBMC in a quarter-sample, MPEG-1 / 2 or obmc_recs-less P picture, H.261, WMV2
+ * mspel, field pictures and field MC in the H.263 family, 4:2:2 / 4:4:4, lowres.  A picture
  * asking for one of them makes the call return -1 with avb200_last_error() set, and nothing is launched.  A record the kernel cannot
  * take (an mv_type outside the family's list, mv_dir above 7, a macroblock outside the picture, a direction whose reference planes are
  * NULL) leaves its macroblock untouched and adds one to *rejected (device uint32).
@@ -522,7 +529,9 @@ int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *recs, size_t n, uint8_t *dst, c
  * [0, 8 * mb_height] x [0, 8 * mb_width]), whatever the records hold: the macroblock-aligned plane plus one row below and one column to
  * the right.  The C code reads that far directly in one case: in a picture narrower (shorter) than 16 samples, FFMAX(h_edge_pos - 16, 0)
  * lets a 16x16 H.263 / MPEG-4 vector at 0 read the reference directly, and its 9-sample chroma block ends one column (row) past the
- * aligned plane.  Elsewhere direct reads may pass h_edge_pos / v_edge_pos but stay inside the aligned plane.  The kernel writes only the
+ * aligned plane.  Elsewhere direct reads may pass h_edge_pos / v_edge_pos but stay inside the aligned plane.  GMC reads less: gmc1_motion
+ * reads a 17 x 17 luma and 9 x 9 chroma window, clamped to [0, h_edge_pos) x [0, v_edge_pos) (halved for chroma) wherever the C code
+ * emulates the edge and else inside the aligned plane; gmc_motion reads only inside [0, h_edge_pos) x [0, v_edge_pos).  The kernel writes only the
  * destination macroblocks of accepted records.
  * Records of one picture run concurrently: a picture holds at most one record per macroblock (two records for the same mb_x, mb_y race,
  * and the result is undefined).  Pictures of one call run concurrently too, so none may read what another writes: a second field that
@@ -535,7 +544,8 @@ typedef struct FFMpvMCRecord {
     uint8_t  mv_type;             /* s->mv_type: 0 16X16, 1 8X8, 2 16X8, 3 FIELD, 4 DMV */
     uint8_t  field_select[2][2];  /* s->field_select */
     int16_t  mv[2][4][2];         /* s->mv */
-    uint8_t  pad[2];
+    uint8_t  mcsel;               /* s->mcsel when ff_mpv_reconstruct_mb runs (mpeg4videodec.c:1221-1227, :1333-1336); read in S-VOPs only */
+    uint8_t  pad;
 } FFMpvMCRecord;
 /* H.263 overlapped block motion compensation (Annex F; Intel H.263; RV10 micro-version 2): apply_obmc (mpegvideo_motion.c:643-728), which
  * replaces ff_mpv_motion's prediction in a P picture with obmc set.  It reads current_picture.motion_val[0] and mb_type at the moment the
@@ -567,6 +577,9 @@ typedef struct FFMpvMCPicture {
     const FFMpvMCRecord *recs;          /* device; at most one record per macroblock */
     size_t n_recs;
     const FFMpvOBMCRecord *obmc_recs;   /* device, one per record in the same order, read when obmc is set in a P picture; else NULL */
+    /* read when sprite is set: the MpegEncContext fields as mpeg4_decode_sprite_trajectory leaves them */
+    int sprite_warping_accuracy, real_sprite_warping_points;
+    int sprite_offset[2][2], sprite_delta[2][2];
 } FFMpvMCPicture;
 int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, int n_pictures, uint32_t *rejected, void *stream);
 
@@ -789,6 +802,11 @@ void ff_qpeldsp_init_cuda(QpelDSPContext *c);
  * line arithmetic; host pointers, the 4 x 8 samples the C function reads around src (two before it) staged and written back.  A qscale
  * outside 0..31, where the C function would read past its strength table, leaves the samples untouched. */
 void ff_h263dsp_init_cuda(H263DSPContext *c);
+/* MpegVideoDSPContext (libavcodec/mpegvideodsp.c:110-119): gmc1 (gmc1_c) and gmc (ff_gmc_c) as a batch of one through the GMC
+ * arithmetic of ff_mpv_motion_batch_cuda; host pointers.  gmc1 stages the 9 x (h + 1) samples it reads at src; gmc stages the
+ * bounding rectangle of the positions its block's four corners map to, clamped to [0, width) x [0, height) of the plane at src (the
+ * whole plane where a corner leaves int32), and writes the 8 x h block back. */
+void ff_mpegvideodsp_init_cuda(MpegVideoDSPContext *c);
 /* libavcodec/fft_template.c:152-159, mdct_template.c:58-66 (same shape as ff_fft_init_x86 / ff_mdct_init_x86): called after
  * ff_fft_init / ff_mdct_init filled the context.  fft_permute stays the reference's; the CUDA fft_calc accepts its revtab
  * order, the MDCT slots use the context's own tcos / tsin tables. */

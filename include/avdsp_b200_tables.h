@@ -139,6 +139,13 @@ typedef struct H263DSPContext {
     void (*h263_v_loop_filter)(uint8_t *src, int stride, int qscale);
 } H263DSPContext;
 
+/* ---- libavcodec/mpegvideodsp.h:27-41 ---- */
+typedef struct MpegVideoDSPContext {
+    void (*gmc1)(uint8_t *dst, uint8_t *src, int srcStride, int h, int x16, int y16, int rounder);
+    void (*gmc)(uint8_t *dst, uint8_t *src, int stride, int h, int ox, int oy, int dxx, int dxy, int dyx, int dyy, int shift, int r,
+                int width, int height);
+} MpegVideoDSPContext;
+
 /* ---- libavcodec/h264chroma.h:25-30 ---- */
 typedef void (*h264_chroma_mc_func)(uint8_t *dst, uint8_t *src, ptrdiff_t srcStride, int h, int x, int y);
 typedef struct H264ChromaContext {

@@ -128,6 +128,7 @@ PROTOTYPES = {
     "ff_h264_pred_init_cuda": (None, [vp, i32, i32, i32]),
     "ff_qpeldsp_init_cuda": (None, [vp]),
     "ff_h263dsp_init_cuda": (None, [vp]),
+    "ff_mpegvideodsp_init_cuda": (None, [vp]),
     "ff_pixblockdsp_init_cuda": (None, [vp, C.c_uint]),
     "ff_fft_init_cuda": (None, [vp]),
     "ff_mdct_init_cuda": (None, [vp]),

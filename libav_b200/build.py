@@ -9,6 +9,7 @@
   oracle/_ref/libmpvqref.so     TEST ONLY: the reference's encoder quantisers (plain, trellis, noise reduction), same conditions
   oracle/_ref/libmpvobmcref.so  TEST ONLY: the reference's H.263 overlapped block motion compensation (apply_obmc), same conditions
   oracle/_ref/libh263ref.so     TEST ONLY: the reference's H.263 deblocking filter (H263DSPContext, ff_h263_loop_filter), same conditions
+  oracle/_ref/libmpvgmcref.so   TEST ONLY: the reference's motion compensation of MPEG-4 S-VOPs (GMC, MpegVideoDSPContext), same conditions
 All outputs are in-tree so they travel to the GPU box with the snapshot.
 """
 import glob
@@ -82,12 +83,14 @@ def build_oracle_port(force=False):
 
 def build_oracle_ref(force=False):
     """Compile the reference's own C sources (read in place) with oracle/refbuild/Makefile: libavref.so, its timing-only SIMD
-    flavour and the satellite libraries of single features, all in one make run."""
+    flavour and the satellite libraries of single features, all in one make run; then the S-VOP library with mpvgmc.mk, which takes
+    its rules from that Makefile."""
     if not os.path.isdir(REFERENCE):
         return ORACLE_REF if os.path.exists(ORACLE_REF) else None
     if force:
         shutil.rmtree(os.path.join(ROOT, "oracle", "_ref"), ignore_errors=True)
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "REF=" + REFERENCE])
+    _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvgmc.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

@@ -1,11 +1,13 @@
 // libav_b200/csrc/mpv_mc.cu -- batched mpegvideo motion compensation (ff_mpv_motion, libavcodec/mpegvideo_motion.c) and the picture flush
 // point of an MPEG-1 / MPEG-2 / H.263 / MPEG-4 decoder back-end.
 //
-// One warp per macroblock record, one lane per destination column (mpv_mc_block.cuh; OBMC pictures in their own kernel, mpv_obmc.cuh).  Up to MPV_PICS_PER_LAUNCH pictures travel as
+// One warp per macroblock record, one lane per destination column (mpv_mc_block.cuh; OBMC pictures and S-VOPs in kernels of their own,
+// mpv_obmc.cuh and mpv_gmc.cuh).  Up to MPV_PICS_PER_LAUNCH pictures travel as
 // kernel parameters; a warp finds its picture by scanning their record offsets.  The pictures' checks are all made on the host before
 // anything is launched, so a refused call leaves the destination as it was.
 #include "mpv_mc_block.cuh"
 #include "mpv_obmc.cuh"
+#include "mpv_gmc.cuh"
 #include "h263_lf.cuh"
 #include <algorithm>
 
@@ -63,6 +65,31 @@ __global__ void __launch_bounds__(128) mpv_obmc_kernel(const __grid_constant__ M
     mpv_obmc_lane(P, r, o, L.weights, threadIdx.x & 31);
 }
 
+// S-VOPs (sprite set): the same walk, with each picture's sprite parameters and the records' mcsel
+struct MpvGmcLaunch {
+    MpvMcPic pic[MPV_PICS_PER_LAUNCH];
+    MpvGmcParams gmc[MPV_PICS_PER_LAUNCH];
+    const FFMpvMCRecord *recs[MPV_PICS_PER_LAUNCH];
+    unsigned long long start[MPV_PICS_PER_LAUNCH + 1];
+    int n;
+    uint32_t *rejected;
+};
+
+__global__ void __launch_bounds__(128) mpv_gmc_kernel(const __grid_constant__ MpvGmcLaunch L)
+{
+    const unsigned long long w = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (w >= L.start[L.n]) return;
+    int p = 0;
+    while (p + 1 < L.n && w >= L.start[p + 1]) p++;
+    const MpvMcPic &P = L.pic[p];
+    const FFMpvMCRecord r = L.recs[p][w - L.start[p]];
+    if (mpv_mc_reject(P, r)) {
+        if ((threadIdx.x & 31) == 0) atomicAdd(L.rejected, 1u);
+        return;
+    }
+    mpv_gmc_lane(P, L.gmc[p], r, threadIdx.x & 31);
+}
+
 namespace {
 
 int refuse(const char *msg) { set_error_msg("ff_mpv_motion_batch_cuda", msg); return -1; }
@@ -73,6 +100,19 @@ const uint8_t *frame_base(const FFMpvMCPicture &q) { return q.dest[0] - (q.pictu
 // apply_obmc runs instead of ff_mpv_motion (mpegvideo_motion.c:829-831)
 bool mpv_obmc_picture(const FFMpvMCPicture &q) { return q.obmc && !q.b_picture; }
 
+// the kernel a picture goes to: 0 plain, 1 OBMC, 2 GMC (an accepted sprite picture is never an OBMC one)
+int mpv_kernel_of(const FFMpvMCPicture &q) { return q.sprite ? 2 : mpv_obmc_picture(q) ? 1 : 0; }
+
+MpvGmcParams mpv_gmc_params(const FFMpvMCPicture &q)
+{
+    MpvGmcParams G;
+    G.acc = q.sprite_warping_accuracy;
+    G.pts = q.real_sprite_warping_points;
+    memcpy(G.off, q.sprite_offset, sizeof(G.off));
+    memcpy(G.delta, q.sprite_delta, sizeof(G.delta));
+    return G;
+}
+
 // the picture-level checks; fills the kernel's view of the picture
 int mpv_picture(const FFMpvMCPicture &q, MpvMcPic &P)
 {
@@ -80,7 +120,10 @@ int mpv_picture(const FFMpvMCPicture &q, MpvMcPic &P)
     if (q.out_format != 0 && q.out_format != 2) return refuse("out_format must be 0 (MPEG-1 / MPEG-2) or 2 (H.263 / MPEG-4)");
     if (q.obmc && !q.b_picture && (q.out_format != 2 || q.quarter_sample || (q.n_recs && !q.obmc_recs)))
         return refuse("OBMC is supported in half-sample H.263-family P pictures with obmc_recs only");
-    if (q.sprite) return refuse("GMC / sprite pictures are not supported");
+    if (q.sprite && (q.out_format != 2 || q.picture_structure != 3 || q.b_picture || q.obmc || q.real_sprite_warping_points < 1 ||
+                     q.real_sprite_warping_points > 3 || q.sprite_warping_accuracy < 0 || q.sprite_warping_accuracy > 3))
+        return refuse("GMC / sprite pictures are supported as MPEG-4 frame S-VOPs without OBMC, with real_sprite_warping_points 1..3 "
+                      "and sprite_warping_accuracy 0..3 only");
     if (q.mspel) return refuse("WMV2 mspel is not supported");
     if (q.lowres) return refuse("lowres is not supported");
     if (q.chroma_format != 1) return refuse("only 4:2:0 chroma is supported");
@@ -140,16 +183,18 @@ extern "C" int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pics, int n, uint3
         }
     if (!rc) {
         enter();
-        // the plain pictures, then the OBMC ones in launches of their own; pictures of a call are independent
-        int *order = new int[n], n_plain = 0;
-        for (int i = 0; i < n; i++)
-            if (!mpv_obmc_picture(pics[i])) order[n_plain++] = i;
-        for (int i = 0, k = n_plain; i < n; i++)
-            if (mpv_obmc_picture(pics[i])) order[k++] = i;
-        for (int g = 0; g < n_plain && !rc; g += MPV_PICS_PER_LAUNCH) {
+        // the plain pictures, then the OBMC ones, then the S-VOPs, each kind in launches of its own; pictures of a call are independent
+        int *order = new int[n], first[4] = { 0, 0, 0, 0 };
+        for (int k = 0, m = 0; k < 3; k++) {
+            first[k] = m;
+            for (int i = 0; i < n; i++)
+                if (mpv_kernel_of(pics[i]) == k) order[m++] = i;
+            first[k + 1] = m;
+        }
+        for (int g = first[0]; g < first[1] && !rc; g += MPV_PICS_PER_LAUNCH) {
             MpvMcLaunch L;
             memset(&L, 0, sizeof(L));
-            L.n = n_plain - g < MPV_PICS_PER_LAUNCH ? n_plain - g : MPV_PICS_PER_LAUNCH;
+            L.n = first[1] - g < MPV_PICS_PER_LAUNCH ? first[1] - g : MPV_PICS_PER_LAUNCH;
             L.rejected = rejected;
             for (int p = 0; p < L.n; p++) {
                 L.pic[p] = P[order[g + p]];
@@ -161,10 +206,10 @@ extern "C" int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pics, int n, uint3
             AVB_LAUNCH(mpv_mc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
             rc = check_launch("ff_mpv_motion_batch_cuda");
         }
-        for (int g = n_plain; g < n && !rc; g += MPV_PICS_PER_LAUNCH) {
+        for (int g = first[1]; g < first[2] && !rc; g += MPV_PICS_PER_LAUNCH) {
             MpvObmcLaunch L;
             memset(&L, 0, sizeof(L));
-            L.n = n - g < MPV_PICS_PER_LAUNCH ? n - g : MPV_PICS_PER_LAUNCH;
+            L.n = first[2] - g < MPV_PICS_PER_LAUNCH ? first[2] - g : MPV_PICS_PER_LAUNCH;
             L.rejected = rejected;
             memcpy(L.weights, mpv_obmc_weights, sizeof(L.weights));
             for (int p = 0; p < L.n; p++) {
@@ -176,6 +221,22 @@ extern "C" int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pics, int n, uint3
             const unsigned long long warps = L.start[L.n];
             if (!warps) continue;
             AVB_LAUNCH(mpv_obmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
+            rc = check_launch("ff_mpv_motion_batch_cuda");
+        }
+        for (int g = first[2]; g < first[3] && !rc; g += MPV_PICS_PER_LAUNCH) {
+            MpvGmcLaunch L;
+            memset(&L, 0, sizeof(L));
+            L.n = first[3] - g < MPV_PICS_PER_LAUNCH ? first[3] - g : MPV_PICS_PER_LAUNCH;
+            L.rejected = rejected;
+            for (int p = 0; p < L.n; p++) {
+                L.pic[p] = P[order[g + p]];
+                L.gmc[p] = mpv_gmc_params(pics[order[g + p]]);
+                L.recs[p] = pics[order[g + p]].recs;
+                L.start[p + 1] = L.start[p] + pics[order[g + p]].n_recs;
+            }
+            const unsigned long long warps = L.start[L.n];
+            if (!warps) continue;
+            AVB_LAUNCH(mpv_gmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
             rc = check_launch("ff_mpv_motion_batch_cuda");
         }
         delete[] order;

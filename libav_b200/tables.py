@@ -69,6 +69,14 @@ class H263DSPContext(C.Structure):          # libavcodec/h263dsp.h:26-29
     _fields_ = [("h263_h_loop_filter", h263_loop_filter_func), ("h263_v_loop_filter", h263_loop_filter_func)]
 
 
+gmc1_func = C.CFUNCTYPE(None, u8p, u8p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)
+gmc_func = C.CFUNCTYPE(None, u8p, u8p, *([C.c_int] * 12))
+
+
+class MpegVideoDSPContext(C.Structure):     # libavcodec/mpegvideodsp.h:27-41
+    _fields_ = [("gmc1", gmc1_func), ("gmc", gmc_func)]
+
+
 qpel_mc_func = C.CFUNCTYPE(None, u8p, u8p, pd)
 
 
@@ -145,7 +153,9 @@ class FFMpvMCPicture(C.Structure):
                 ("h_edge_pos", C.c_int), ("v_edge_pos", C.c_int), ("out_format", C.c_int), ("picture_structure", C.c_int),
                 ("first_field", C.c_int), ("b_picture", C.c_int), ("no_rounding", C.c_int), ("quarter_sample", C.c_int),
                 ("workaround_bugs", C.c_int), ("chroma_format", C.c_int), ("obmc", C.c_int), ("sprite", C.c_int), ("mspel", C.c_int),
-                ("lowres", C.c_int), ("recs", C.c_void_p), ("n_recs", C.c_size_t), ("obmc_recs", C.c_void_p)]
+                ("lowres", C.c_int), ("recs", C.c_void_p), ("n_recs", C.c_size_t), ("obmc_recs", C.c_void_p),
+                ("sprite_warping_accuracy", C.c_int), ("real_sprite_warping_points", C.c_int),
+                ("sprite_offset", (C.c_int * 2) * 2), ("sprite_delta", (C.c_int * 2) * 2)]
 
 
 class FFMpvResidualBatch(C.Structure):

@@ -4,19 +4,22 @@ motion compensation, then the residual batches) on HBM-resident batches.
 
   python tools/mpv_mc_bench.py [--rounds 7] [--steps 50] [--warmup 5] [--out FILE.json]
 
-Two batches of sixteen 1920x1088 pictures, records generated with mostly small vectors (tests/mpv_mc_cases.py); 8 % of the macroblocks are
+Three batches of sixteen 1920x1088 pictures, records generated with mostly small vectors (tests/mpv_mc_cases.py); 8 % of the macroblocks are
 intra (no MC, six coded blocks), each block of an inter macroblock is coded at probability 0.5 (tests/mpv_mc_cases.py decoder_residual):
   mpeg2  MPEG-2: frame P and B pictures (16X16, FIELD, DMV; half the macroblocks with field DCT) and field pictures (FIELD, 16X8, DMV),
          first and second fields; simple IDCT, idct_put for intra and idct_add for inter blocks
   mpeg4  MPEG-4 ASP as Xvid writes it: quarter-sample P and B pictures, 16X16 and 4MV, bi-predicted 8x8 records like B-direct; the Xvid
          IDCT, intra blocks through the fused h263_intra dequantiser, inter blocks added
+  mpeg4_gmc  MPEG-4 ASP S-VOPs with GMC (tests/mpv_gmc_cases.py): 2- and 3-point warps from random sprite trajectories, about 70 % of the
+         macroblocks mcsel 16X16 (four in five of them skipped: no residual), the rest quarter-sample 16X16 and 4MV; residual as mpeg4
 The residual batches run without `clear`, so every timed flush transforms the same coefficients.  The arms `mc` (the motion compensation
 alone) and `flush` alternate within each round; a round times `steps` calls with CUDA events after `warmup` untimed ones.  Printed per
 batch and arm: the median and best ms per call, the spread (max - min) / median over the rounds, Mpixel/s of predicted pictures, and the
 algorithmic bytes over the median time as a fraction of the H100 SXM data sheet's 3.35 TB/s.  Bytes: per macroblock and direction 384 B
 of prediction read and 384 B written, plus the 44-byte record; per residual block 128 B of coefficients read and 64 B of pixels written
 (+ 64 B read for add, + 4 B of dequantiser record).  The CPU figure is the reference's own ff_mpv_motion (oracle/_ref/libmpvmcref.so,
-portable C) over the same records on all host cores, one picture per thread (motion compensation only).  After timing, every picture is
+portable C; ref_mpvmc_gmc_picture of oracle/_ref/libmpvgmcref.so for the S-VOPs) over the same records on all host cores, one picture per thread (motion compensation
+only).  After timing, every picture is
 rebuilt from its original bytes by one flush and compared with the chained checker: the reference's MC, then the IDCT and inverse
 quantiser oracles over the same batches.  The card's name, power limit and maximum SM clock come from a read-only nvidia-smi query and are
 printed with the numbers.
@@ -47,8 +50,42 @@ def card():
     return out.splitlines()[0] if out else "unknown"
 
 
+def gmc_batch(checker):
+    """sixteen S-VOPs; the residual of skipped mcsel macroblocks is dropped"""
+    import mpv_gmc_cases as G
+    import mpv_mc_cases as M
+    pics, skipped = [], []
+    for i in range(16):
+        rng = np.random.default_rng(2000 + i)
+        pic = M.Picture(rng, 2, 120, 68, no_rnd=(i >> 1) & 1, qpel=1, width=1920, height=1080)
+        old = M.make_records(rng, pic, far=0.0, edge=0.02, types=[M.T16X16, M.T8X8])
+        recs = np.zeros(len(old), G.REC)
+        for name in M.REC.names:
+            if name != "pad":
+                recs[name] = old[name]
+        recs["mv_dir"] = 1
+        recs["mcsel"] = rng.random(len(recs)) < 0.7
+        recs["mv_type"][recs["mcsel"] == 1] = M.T16X16
+        pic.recs = recs
+        pic.sprite = G.random_params(rng, 1920, 1080, 120, 68, 1920, 1080, pts=2 + (i & 1), scale=16)
+        skipped.append({(int(r["mb_x"]), int(r["mb_y"])) for r in recs if r["mcsel"] and rng.random() < 0.8})
+        pics.append(pic)
+    residual = M.decoder_residual(checker, pics, np.random.default_rng(9), xvid=True, clear=0)
+    for b in residual:
+        if b["dq"] >= 0:
+            continue                                         # intra blocks
+        pic = pics[b["pi"]]
+        ls = pic.p["linesize"] if b["pl"] == 0 else pic.p["uvlinesize"]
+        mb = 16 if b["pl"] == 0 else 8
+        keep = np.array([((int(o) % ls) // mb, (int(o) // ls) // mb) not in skipped[b["pi"]] for o in b["off"]], bool)
+        b["off"], b["blocks"], b["rec"] = np.ascontiguousarray(b["off"][keep]), np.ascontiguousarray(b["blocks"][keep]), b["rec"][keep]
+    return pics, [b for b in residual if len(b["off"])]
+
+
 def batch(kind, checker):
     import mpv_mc_cases as M
+    if kind == "mpeg4_gmc":
+        return gmc_batch(checker)
     pics = []
     for i in range(16):
         rng = np.random.default_rng(1000 * (kind == "mpeg4") + i)
@@ -73,16 +110,17 @@ def main():
     import libav_b200._lib as L
     from libav_b200 import device
     from oracle import loader
+    import mpv_gmc_cases as G
     import mpv_mc_cases as M
     L.init(0)
-    ref = M.ref_lib()
     checker = loader.ref() or loader.port()
-    mc_checker = M.checker_lib()
     results = {"card": card()}
     print("card: %s" % results["card"])
-    for kind in ("mpeg2", "mpeg4"):
+    for kind in ("mpeg2", "mpeg4", "mpeg4_gmc"):
+        C_ = G if kind == "mpeg4_gmc" else M          # the S-VOPs' reference, checker and device pictures
+        ref, mc_checker = C_.ref_lib(), C_.checker_lib()
         pics, residual = batch(kind, checker)
-        g = M.GpuPictures(pics)
+        g = G.GpuSvops(pics) if kind == "mpeg4_gmc" else M.GpuPictures(pics)
         res = M.GpuResidual(g, residual)
         work = res.work(g)
         n_mb_dir = sum(int(((p.recs["mv_dir"] & 1) != 0).sum() + ((p.recs["mv_dir"] & 2) != 0).sum()) for p in pics)
@@ -115,10 +153,10 @@ def main():
         if ref is not None:
             t0 = time.perf_counter()
             with cf.ThreadPoolExecutor(os.cpu_count()) as ex:
-                list(ex.map(lambda p: M.run_ref(ref, p), pics))
+                list(ex.map(lambda p: C_.run_ref(ref, p), pics))
             r["cpu_mc_ms"], r["cpu_threads"] = (time.perf_counter() - t0) * 1e3, os.cpu_count()
         # verification: one flush over the original pictures against the chained checker
-        want = [M.run_ref(mc_checker, p) for p in pics]
+        want = [C_.run_ref(mc_checker, p) for p in pics]
         M.apply_residual(checker, M.xvid_checker(), want, residual)
         for fr, pic in zip(g.frames, pics):
             for b, a in zip(fr, pic.frame):
