@@ -501,14 +501,18 @@ int ff_hpel_batch_cuda(const FFHpelRecord *recs, size_t n, uint8_t *dst, const u
 typedef struct FFQpelRecord { uint32_t dst_off, src_off; uint8_t kind, sidx, mc, pad; } FFQpelRecord;
 int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *recs, size_t n, uint8_t *dst, const uint8_t *src, ptrdiff_t stride, void *stream);
 
-/* ---- mpegvideo motion compensation (MPEG-1 / MPEG-2, H.263 / MPEG-4 part 2; 8 bit 4:2:0) ------------------------------------------------
+/* ---- mpegvideo motion compensation (MPEG-1 / MPEG-2 4:2:0 / 4:2:2 / 4:4:4, H.263 / MPEG-4 part 2 4:2:0; 8 bit) ---------------------------
  * ff_mpv_motion() (libavcodec/mpegvideo_motion.c:814-968) for every direction of a macroblock, in ff_mpv_reconstruct_mb's order
  * (mpegvideo.c:1548-1578): the forward prediction with put (put_no_rnd when no_rounding is set in a P picture), then the backward one
  * with avg.  One record per inter macroblock, its fields named after the MpegEncContext fields the C function reads.
  *   MPEG-1 / MPEG-2 (out_format 0): 16X16 in frame pictures; FIELD in frame and field pictures; 16X8 in field pictures; DMV in both.
- *     A vector whose block leaves [0, h_edge_pos) x [0, v_edge_pos) skips that mpeg_motion call, exactly like the C code (:333-342).
+ *     Chroma 4:2:0, 4:2:2 or 4:4:4 (chroma_format 1, 2, 3: mpeg_motion_internal's chroma cases, :307-326).  A vector whose luma block
+ *     leaves [0, h_edge_pos) x [0, v_edge_pos) skips that mpeg_motion call, chroma included, exactly like the C code (:333-342).
  *   H.263 / MPEG-4 (out_format 2): 16X16 half- and quarter-sample, 8X8 (4MV) half- and quarter-sample, with the reference's edge
- *     emulation where it emulates (clamped addressing) and direct reads where it reads directly.
+ *     emulation where it emulates (clamped addressing) and direct reads where it reads directly.  In an interlaced MPEG-4 picture
+ *     (interlaced set) also FIELD: mpeg_motion_field for each parity (FF_BUG_HPEL_CHROMA's chroma vector when workaround_bugs has it),
+ *     or, quarter-sample, qpel_motion with field_based (two 8x8 qpel ops per field).  Their edge emulation works in frame rows, as
+ *     emulated_edge_mc does: field row i of parity f reads frame row av_clip(2 * (src_y + i) + f, 0, v_edge_pos - 1).
  * OBMC: a P picture with obmc set (out_format 2, half-sample, obmc_recs given) runs apply_obmc for each record instead, from its
  *   FFMpvOBMCRecord: the four 8x8 luma blocks as put_obmc weighted sums of hpel_motion predictions (put_no_rnd under no_rounding), chroma
  *   through chroma_4mv_motion with the sum of the four own vectors -- also for a 16X16 macroblock.  Its records must be forward-only
@@ -520,14 +524,15 @@ int ff_mpeg4_qpel_batch_cuda(const FFQpelRecord *recs, size_t n, uint8_t *dst, c
  *   The sprite fields must be those mpeg4_decode_sprite_trajectory (mpeg4videodec.c:168-385) leaves: the C arithmetic, which the kernel
  *   follows, is only defined where gmc_motion's and ff_gmc_c's intermediates fit int32 (the kernel's affine map is that arithmetic
  *   mod 2^32 all the same).
- * Refused: static sprites and any other sprite picture, OBMC in a quarter-sample, MPEG-1 / 2 or obmc_recs-less P picture, H.261, WMV2
- * mspel, field pictures and field MC in the H.263 family, 4:2:2 / 4:4:4, lowres.  A picture
+ * Refused: static sprites and any other sprite picture, OBMC in a quarter-sample, MPEG-1 / 2, obmc_recs-less or interlaced P picture,
+ * H.261, WMV2 mspel, field pictures in the H.263 family, chroma_format outside 1..3 or other than 1 in the H.263 family, lowres.  A picture
  * asking for one of them makes the call return -1 with avb200_last_error() set, and nothing is launched.  A record the kernel cannot
- * take (an mv_type outside the family's list, mv_dir above 7, a macroblock outside the picture, a direction whose reference planes are
- * NULL) leaves its macroblock untouched and adds one to *rejected (device uint32).
+ * take (an mv_type outside the family's list -- FIELD counts as outside it in an H.263-family picture without interlaced, 16X8 and DMV
+ * always --, mv_dir above 7, a macroblock outside the picture, a direction whose reference planes are NULL) leaves its macroblock
+ * untouched and adds one to *rejected (device uint32).
  * Memory: the kernel reads each reference plane only inside rows [0, 16 * mb_height] and columns [0, 16 * mb_width] (chroma
- * [0, 8 * mb_height] x [0, 8 * mb_width]), whatever the records hold: the macroblock-aligned plane plus one row below and one column to
- * the right.  The C code reads that far directly in one case: in a picture narrower (shorter) than 16 samples, FFMAX(h_edge_pos - 16, 0)
+ * [0, (16 >> chroma_y_shift) * mb_height] x [0, (16 >> chroma_x_shift) * mb_width]: 8 x 8 per macroblock in 4:2:0, 8 wide and 16 high in
+ * 4:2:2, 16 x 16 in 4:4:4), whatever the records hold: the macroblock-aligned plane plus one row below and one column to the right.  The C code reads that far directly in one case: in a picture narrower (shorter) than 16 samples, FFMAX(h_edge_pos - 16, 0)
  * lets a 16x16 H.263 / MPEG-4 vector at 0 read the reference directly, and its 9-sample chroma block ends one column (row) past the
  * aligned plane.  Elsewhere direct reads may pass h_edge_pos / v_edge_pos but stay inside the aligned plane.  GMC reads less: gmc1_motion
  * reads a 17 x 17 luma and 9 x 9 chroma window, clamped to [0, h_edge_pos) x [0, v_edge_pos) (halved for chroma) wherever the C code
@@ -572,7 +577,7 @@ typedef struct FFMpvMCPicture {
     int picture_structure;              /* 1 top field, 2 bottom field, 3 frame */
     int first_field, b_picture;         /* s->first_field; s->pict_type == AV_PICTURE_TYPE_B */
     int no_rounding, quarter_sample, workaround_bugs;
-    int chroma_format;                  /* s->chroma_format: 1 (4:2:0) */
+    int chroma_format;                  /* s->chroma_format: 1 (4:2:0); 2 (4:2:2) or 3 (4:4:4) with out_format 0 only */
     int obmc, sprite, mspel, lowres;    /* s->obmc; s->pict_type == AV_PICTURE_TYPE_S; s->mspel; avctx->lowres: must be 0 */
     const FFMpvMCRecord *recs;          /* device; at most one record per macroblock */
     size_t n_recs;
@@ -580,6 +585,7 @@ typedef struct FFMpvMCPicture {
     /* read when sprite is set: the MpegEncContext fields as mpeg4_decode_sprite_trajectory leaves them */
     int sprite_warping_accuracy, real_sprite_warping_points;
     int sprite_offset[2][2], sprite_delta[2][2];
+    int interlaced;                     /* !s->progressive_sequence, read in out_format 2 only: FIELD records of the frame picture are taken */
 } FFMpvMCPicture;
 int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, int n_pictures, uint32_t *rejected, void *stream);
 

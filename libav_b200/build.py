@@ -83,14 +83,15 @@ def build_oracle_port(force=False):
 
 def build_oracle_ref(force=False):
     """Compile the reference's own C sources (read in place) with oracle/refbuild/Makefile: libavref.so, its timing-only SIMD
-    flavour and the satellite libraries of single features, all in one make run; then the S-VOP library with mpvgmc.mk, which takes
-    its rules from that Makefile."""
+    flavour and the satellite libraries of single features, all in one make run; then the S-VOP library with mpvgmc.mk and
+    the any-chroma-format MPEG-2 library with mpvcf.mk, which take their rules from that Makefile."""
     if not os.path.isdir(REFERENCE):
         return ORACLE_REF if os.path.exists(ORACLE_REF) else None
     if force:
         shutil.rmtree(os.path.join(ROOT, "oracle", "_ref"), ignore_errors=True)
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "REF=" + REFERENCE])
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvgmc.mk", "REF=" + REFERENCE])
+    _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "mpvcf.mk", "REF=" + REFERENCE])
     return ORACLE_REF
 
 

@@ -1,8 +1,8 @@
 // libav_b200/csrc/mpv_gmc.cuh -- MPEG-4 global motion compensation: gmc1_motion / gmc_motion (libavcodec/mpegvideo_motion.c:37-190) with
 // the MpegVideoDSPContext arithmetic they call (gmc1_c, ff_gmc_c: libavcodec/mpegvideodsp.c:24-108), one lane per destination column like
-// mpv_mc_block.cuh, whose fetch / store / hpel helpers and plain body it reuses.  A separate kernel (mpv_gmc_kernel in mpv_mc.cu) runs
-// S-VOPs, so the plain MC kernel is unchanged.  Lanes never communicate: tests/hostsim/ runs the body.  The slot kernel of
-// MpegVideoDSPContext (mpegvideodsp.cu) shares the two sample functions.
+// mpv_mc_block.cuh, whose fetch / store / hpel helpers and plain body it reuses.  A separate kernel (mpv_gmc_kernel in mpv_mc.cu;
+// mpv_gmc_ilace_kernel for interlaced ones) runs S-VOPs, so the plain MC kernel is unchanged.  Lanes never communicate: tests/hostsim/ runs
+// the body.  The slot kernel of MpegVideoDSPContext (mpegvideodsp.cu) shares the two sample functions.
 #pragma once
 #include "mpv_mc_block.cuh"
 
@@ -90,11 +90,12 @@ __device__ __forceinline__ void mpv_gmc_motion(const MpvMcPic &P, const MpvGmcPa
 }
 
 // ff_mpv_motion for a record of an S-VOP: a 16X16 record with mcsel runs gmc1_motion / gmc_motion (mpegvideo_motion.c:834-843) with put
-// for each direction it names, every other record the plain body
+// for each direction it names, every other record the plain body (IL: that of an interlaced picture, FIELD records included)
+template <int IL = 0>
 __device__ __forceinline__ void mpv_gmc_lane(const MpvMcPic &P, const MpvGmcParams &G, const FFMpvMCRecord &r, int lane)
 {
     if (r.mv_type != MPV_MC_16X16 || !r.mcsel) {
-        mpv_mc_lane(P, r, lane);
+        mpv_mc_lane<1, IL>(P, r, lane);
         return;
     }
     MpvLane L;

@@ -2,7 +2,8 @@
 // point of an MPEG-1 / MPEG-2 / H.263 / MPEG-4 decoder back-end.
 //
 // One warp per macroblock record, one lane per destination column (mpv_mc_block.cuh; OBMC pictures and S-VOPs in kernels of their own,
-// mpv_obmc.cuh and mpv_gmc.cuh).  Up to MPV_PICS_PER_LAUNCH pictures travel as
+// mpv_obmc.cuh and mpv_gmc.cuh; MPEG-2 4:2:2 and 4:4:4 pictures and interlaced MPEG-4 pictures in instances of the same body that run in
+// launches of their own, so progressive 4:2:0 pictures run the code they ran before).  Up to MPV_PICS_PER_LAUNCH pictures travel as
 // kernel parameters; a warp finds its picture by scanning their record offsets.  The pictures' checks are all made on the host before
 // anything is launched, so a refused call leaves the destination as it was.
 #include "mpv_mc_block.cuh"
@@ -23,7 +24,9 @@ struct MpvMcLaunch {
     uint32_t *rejected;
 };
 
-__global__ void __launch_bounds__(128) mpv_mc_kernel(const __grid_constant__ MpvMcLaunch L)
+// the warp's record of a launch, the picture kind's body on it (CF, IL: mpv_mc_block.cuh)
+template <int CF, int IL>
+__device__ __forceinline__ void mpv_mc_warp(const MpvMcLaunch &L)
 {
     const unsigned long long w = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (w >= L.start[L.n]) return;
@@ -31,12 +34,21 @@ __global__ void __launch_bounds__(128) mpv_mc_kernel(const __grid_constant__ Mpv
     while (p + 1 < L.n && w >= L.start[p + 1]) p++;
     const MpvMcPic &P = L.pic[p];
     const FFMpvMCRecord r = L.recs[p][w - L.start[p]];
-    if (mpv_mc_reject(P, r)) {
+    if (mpv_mc_reject_kind<IL>(P, r)) {
         if ((threadIdx.x & 31) == 0) atomicAdd(L.rejected, 1u);
         return;
     }
-    mpv_mc_lane(P, r, threadIdx.x & 31);
+    mpv_mc_lane<CF, IL>(P, r, threadIdx.x & 31);
 }
+
+__global__ void __launch_bounds__(128) mpv_mc_kernel(const __grid_constant__ MpvMcLaunch L) { mpv_mc_warp<1, 0>(L); }
+
+// MPEG-2 4:2:2 (CF 2) and 4:4:4 (CF 3) pictures
+template <int CF>
+__global__ void __launch_bounds__(128) mpv_mc_chroma_kernel(const __grid_constant__ MpvMcLaunch L) { mpv_mc_warp<CF, 0>(L); }
+
+// interlaced MPEG-4 pictures (interlaced set in out_format 2) other than S-VOPs
+__global__ void __launch_bounds__(128) mpv_mc_ilace_kernel(const __grid_constant__ MpvMcLaunch L) { mpv_mc_warp<1, 1>(L); }
 
 // OBMC pictures (obmc set in a P picture): the same walk, with each record's FFMpvOBMCRecord and put_obmc's weights
 struct MpvObmcLaunch {
@@ -75,7 +87,8 @@ struct MpvGmcLaunch {
     uint32_t *rejected;
 };
 
-__global__ void __launch_bounds__(128) mpv_gmc_kernel(const __grid_constant__ MpvGmcLaunch L)
+template <int IL>
+__device__ __forceinline__ void mpv_gmc_warp(const MpvGmcLaunch &L)
 {
     const unsigned long long w = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (w >= L.start[L.n]) return;
@@ -83,12 +96,17 @@ __global__ void __launch_bounds__(128) mpv_gmc_kernel(const __grid_constant__ Mp
     while (p + 1 < L.n && w >= L.start[p + 1]) p++;
     const MpvMcPic &P = L.pic[p];
     const FFMpvMCRecord r = L.recs[p][w - L.start[p]];
-    if (mpv_mc_reject(P, r)) {
+    if (mpv_mc_reject_kind<IL>(P, r)) {
         if ((threadIdx.x & 31) == 0) atomicAdd(L.rejected, 1u);
         return;
     }
-    mpv_gmc_lane(P, L.gmc[p], r, threadIdx.x & 31);
+    mpv_gmc_lane<IL>(P, L.gmc[p], r, threadIdx.x & 31);
 }
+
+__global__ void __launch_bounds__(128) mpv_gmc_kernel(const __grid_constant__ MpvGmcLaunch L) { mpv_gmc_warp<0>(L); }
+
+// interlaced S-VOPs: their non-mcsel records may be FIELD ones
+__global__ void __launch_bounds__(128) mpv_gmc_ilace_kernel(const __grid_constant__ MpvGmcLaunch L) { mpv_gmc_warp<1>(L); }
 
 namespace {
 
@@ -100,8 +118,18 @@ const uint8_t *frame_base(const FFMpvMCPicture &q) { return q.dest[0] - (q.pictu
 // apply_obmc runs instead of ff_mpv_motion (mpegvideo_motion.c:829-831)
 bool mpv_obmc_picture(const FFMpvMCPicture &q) { return q.obmc && !q.b_picture; }
 
-// the kernel a picture goes to: 0 plain, 1 OBMC, 2 GMC (an accepted sprite picture is never an OBMC one)
-int mpv_kernel_of(const FFMpvMCPicture &q) { return q.sprite ? 2 : mpv_obmc_picture(q) ? 1 : 0; }
+// the kernel a picture goes to, in launch order (an accepted sprite picture is never an OBMC one, an accepted OBMC picture never
+// interlaced, and chroma other than 4:2:0 is MPEG-1 / MPEG-2's alone)
+enum { MPV_K_PLAIN, MPV_K_OBMC, MPV_K_GMC, MPV_K_422, MPV_K_444, MPV_K_ILACE, MPV_K_GMC_ILACE, MPV_KINDS };
+
+int mpv_kernel_of(const FFMpvMCPicture &q)
+{
+    const bool il = q.out_format == 2 && q.interlaced;
+    if (q.sprite) return il ? MPV_K_GMC_ILACE : MPV_K_GMC;
+    if (mpv_obmc_picture(q)) return MPV_K_OBMC;
+    if (q.chroma_format != 1) return q.chroma_format == 2 ? MPV_K_422 : MPV_K_444;
+    return il ? MPV_K_ILACE : MPV_K_PLAIN;
+}
 
 MpvGmcParams mpv_gmc_params(const FFMpvMCPicture &q)
 {
@@ -126,14 +154,17 @@ int mpv_picture(const FFMpvMCPicture &q, MpvMcPic &P)
                       "and sprite_warping_accuracy 0..3 only");
     if (q.mspel) return refuse("WMV2 mspel is not supported");
     if (q.lowres) return refuse("lowres is not supported");
-    if (q.chroma_format != 1) return refuse("only 4:2:0 chroma is supported");
+    if (q.chroma_format < 1 || q.chroma_format > 3 || (q.chroma_format != 1 && q.out_format != 0))
+        return refuse("chroma_format must be 1 (4:2:0), or 2 (4:2:2) / 3 (4:4:4) in MPEG-1 / MPEG-2 pictures");
+    if (q.out_format == 2 && q.interlaced && q.obmc && !q.b_picture) return refuse("OBMC is not supported in interlaced P pictures");
     if (q.picture_structure < 1 || q.picture_structure > 3) return refuse("picture_structure must be 1, 2 or 3");
     const bool frame = q.picture_structure == 3, h263 = q.out_format == 2;
     if (h263 && !frame) return refuse("field pictures are not supported in the H.263 family");
     if (q.mb_width <= 0 || q.mb_height <= 0 || q.mb_width > 4096 || q.mb_height > 4096 || (!frame && (q.mb_height & 1)))
         return refuse("bad macroblock dimensions");
-    if (q.linesize < 16 * q.mb_width + 1 || q.uvlinesize < 8 * q.mb_width + 1 || (q.linesize | q.uvlinesize) < 0)
-        return refuse("linesize / uvlinesize must exceed the macroblock-aligned width");
+    const int cx = q.chroma_format != 3, cy = q.chroma_format == 1;    // chroma_x_shift, chroma_y_shift
+    if (q.linesize < 16 * q.mb_width + 1 || q.uvlinesize < (16 >> cx) * q.mb_width + 1 || (q.linesize | q.uvlinesize) < 0)
+        return refuse("linesize / uvlinesize must exceed the macroblock-aligned width of the plane");
     const int k = frame ? 1 : 2;
     if (q.pic_linesize != k * q.linesize || q.pic_uvlinesize != k * q.uvlinesize)
         return refuse("pic_linesize must be linesize (frame pictures) or 2 * linesize (field pictures)");
@@ -156,8 +187,53 @@ int mpv_picture(const FFMpvMCPicture &q, MpvMcPic &P)
     P.h263 = h263; P.structure = q.picture_structure; P.first_field = q.first_field != 0; P.b_pic = q.b_picture != 0;
     P.no_rnd = q.no_rounding != 0; P.bugs = q.workaround_bugs; P.qpel = h263 && q.quarter_sample;
     P.rw[0] = 16 * q.mb_width + 1; P.rh[0] = 16 * q.mb_height + 1;
-    P.rw[1] = 8 * q.mb_width + 1;  P.rh[1] = 8 * q.mb_height + 1;
+    P.rw[1] = (16 >> cx) * q.mb_width + 1; P.rh[1] = (16 >> cy) * q.mb_height + 1;
     return 0;
+}
+
+// the pictures, records and warp starts of one launch of the pictures pics[idx[0..m)]; returns the launch's warps
+template <class Launch>
+unsigned long long mpv_fill(Launch &L, const FFMpvMCPicture *pics, const MpvMcPic *P, const int *idx, int m, uint32_t *rejected)
+{
+    memset(&L, 0, sizeof(L));
+    L.n = m;
+    L.rejected = rejected;
+    for (int p = 0; p < m; p++) {
+        L.pic[p] = P[idx[p]];
+        L.recs[p] = pics[idx[p]].recs;
+        L.start[p + 1] = L.start[p] + pics[idx[p]].n_recs;
+    }
+    return L.start[m];
+}
+
+// one launch of kind k (mpv_kernel_of) over the pictures pics[idx[0..m)], m <= MPV_PICS_PER_LAUNCH
+int mpv_launch(int k, const FFMpvMCPicture *pics, const MpvMcPic *P, const int *idx, int m, uint32_t *rejected, cudaStream_t stream)
+{
+    if (k == MPV_K_OBMC) {
+        MpvObmcLaunch L;
+        const unsigned long long warps = mpv_fill(L, pics, P, idx, m, rejected);
+        if (!warps) return 0;
+        memcpy(L.weights, mpv_obmc_weights, sizeof(L.weights));
+        for (int p = 0; p < m; p++) L.obmc[p] = pics[idx[p]].obmc_recs;
+        AVB_LAUNCH(mpv_obmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, stream)(L);
+    } else if (k == MPV_K_GMC || k == MPV_K_GMC_ILACE) {
+        MpvGmcLaunch L;
+        const unsigned long long warps = mpv_fill(L, pics, P, idx, m, rejected);
+        if (!warps) return 0;
+        for (int p = 0; p < m; p++) L.gmc[p] = mpv_gmc_params(pics[idx[p]]);
+        if (k == MPV_K_GMC) AVB_LAUNCH(mpv_gmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, stream)(L);
+        else                AVB_LAUNCH(mpv_gmc_ilace_kernel, (unsigned)((warps + 3) / 4), 128, 0, stream)(L);
+    } else {
+        MpvMcLaunch L;
+        const unsigned long long warps = mpv_fill(L, pics, P, idx, m, rejected);
+        if (!warps) return 0;
+        const unsigned grid = (unsigned)((warps + 3) / 4);
+        if (k == MPV_K_PLAIN)      AVB_LAUNCH(mpv_mc_kernel, grid, 128, 0, stream)(L);
+        else if (k == MPV_K_422)   AVB_LAUNCH(mpv_mc_chroma_kernel<2>, grid, 128, 0, stream)(L);
+        else if (k == MPV_K_444)   AVB_LAUNCH(mpv_mc_chroma_kernel<3>, grid, 128, 0, stream)(L);
+        else                       AVB_LAUNCH(mpv_mc_ilace_kernel, grid, 128, 0, stream)(L);
+    }
+    return check_launch("ff_mpv_motion_batch_cuda");
 }
 
 }  // namespace
@@ -183,62 +259,17 @@ extern "C" int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pics, int n, uint3
         }
     if (!rc) {
         enter();
-        // the plain pictures, then the OBMC ones, then the S-VOPs, each kind in launches of its own; pictures of a call are independent
-        int *order = new int[n], first[4] = { 0, 0, 0, 0 };
-        for (int k = 0, m = 0; k < 3; k++) {
+        // each kind of picture in launches of its own, in mpv_kernel_of's order; pictures of a call are independent
+        int *order = new int[n], first[MPV_KINDS + 1] = {};
+        for (int k = 0, m = 0; k < MPV_KINDS; k++) {
             first[k] = m;
             for (int i = 0; i < n; i++)
                 if (mpv_kernel_of(pics[i]) == k) order[m++] = i;
             first[k + 1] = m;
         }
-        for (int g = first[0]; g < first[1] && !rc; g += MPV_PICS_PER_LAUNCH) {
-            MpvMcLaunch L;
-            memset(&L, 0, sizeof(L));
-            L.n = first[1] - g < MPV_PICS_PER_LAUNCH ? first[1] - g : MPV_PICS_PER_LAUNCH;
-            L.rejected = rejected;
-            for (int p = 0; p < L.n; p++) {
-                L.pic[p] = P[order[g + p]];
-                L.recs[p] = pics[order[g + p]].recs;
-                L.start[p + 1] = L.start[p] + pics[order[g + p]].n_recs;
-            }
-            const unsigned long long warps = L.start[L.n];
-            if (!warps) continue;
-            AVB_LAUNCH(mpv_mc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
-            rc = check_launch("ff_mpv_motion_batch_cuda");
-        }
-        for (int g = first[1]; g < first[2] && !rc; g += MPV_PICS_PER_LAUNCH) {
-            MpvObmcLaunch L;
-            memset(&L, 0, sizeof(L));
-            L.n = first[2] - g < MPV_PICS_PER_LAUNCH ? first[2] - g : MPV_PICS_PER_LAUNCH;
-            L.rejected = rejected;
-            memcpy(L.weights, mpv_obmc_weights, sizeof(L.weights));
-            for (int p = 0; p < L.n; p++) {
-                L.pic[p] = P[order[g + p]];
-                L.recs[p] = pics[order[g + p]].recs;
-                L.obmc[p] = pics[order[g + p]].obmc_recs;
-                L.start[p + 1] = L.start[p] + pics[order[g + p]].n_recs;
-            }
-            const unsigned long long warps = L.start[L.n];
-            if (!warps) continue;
-            AVB_LAUNCH(mpv_obmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
-            rc = check_launch("ff_mpv_motion_batch_cuda");
-        }
-        for (int g = first[2]; g < first[3] && !rc; g += MPV_PICS_PER_LAUNCH) {
-            MpvGmcLaunch L;
-            memset(&L, 0, sizeof(L));
-            L.n = first[3] - g < MPV_PICS_PER_LAUNCH ? first[3] - g : MPV_PICS_PER_LAUNCH;
-            L.rejected = rejected;
-            for (int p = 0; p < L.n; p++) {
-                L.pic[p] = P[order[g + p]];
-                L.gmc[p] = mpv_gmc_params(pics[order[g + p]]);
-                L.recs[p] = pics[order[g + p]].recs;
-                L.start[p + 1] = L.start[p] + pics[order[g + p]].n_recs;
-            }
-            const unsigned long long warps = L.start[L.n];
-            if (!warps) continue;
-            AVB_LAUNCH(mpv_gmc_kernel, (unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream)(L);
-            rc = check_launch("ff_mpv_motion_batch_cuda");
-        }
+        for (int k = 0; k < MPV_KINDS && !rc; k++)
+            for (int g = first[k]; g < first[k + 1] && !rc; g += MPV_PICS_PER_LAUNCH)
+                rc = mpv_launch(k, pics, P, order + g, std::min(first[k + 1] - g, (int)MPV_PICS_PER_LAUNCH), rejected, (cudaStream_t)stream);
         delete[] order;
     }
     delete[] P;

@@ -155,7 +155,7 @@ class FFMpvMCPicture(C.Structure):
                 ("workaround_bugs", C.c_int), ("chroma_format", C.c_int), ("obmc", C.c_int), ("sprite", C.c_int), ("mspel", C.c_int),
                 ("lowres", C.c_int), ("recs", C.c_void_p), ("n_recs", C.c_size_t), ("obmc_recs", C.c_void_p),
                 ("sprite_warping_accuracy", C.c_int), ("real_sprite_warping_points", C.c_int),
-                ("sprite_offset", (C.c_int * 2) * 2), ("sprite_delta", (C.c_int * 2) * 2)]
+                ("sprite_offset", (C.c_int * 2) * 2), ("sprite_delta", (C.c_int * 2) * 2), ("interlaced", C.c_int)]
 
 
 class FFMpvResidualBatch(C.Structure):

@@ -4,7 +4,7 @@ motion compensation, then the residual batches) on HBM-resident batches.
 
   python tools/mpv_mc_bench.py [--rounds 7] [--steps 50] [--warmup 5] [--out FILE.json]
 
-Three batches of sixteen 1920x1088 pictures, records generated with mostly small vectors (tests/mpv_mc_cases.py); 8 % of the macroblocks are
+Five batches of sixteen 1920x1088 pictures, records generated with mostly small vectors (tests/mpv_mc_cases.py); 8 % of the macroblocks are
 intra (no MC, six coded blocks), each block of an inter macroblock is coded at probability 0.5 (tests/mpv_mc_cases.py decoder_residual):
   mpeg2  MPEG-2: frame P and B pictures (16X16, FIELD, DMV; half the macroblocks with field DCT) and field pictures (FIELD, 16X8, DMV),
          first and second fields; simple IDCT, idct_put for intra and idct_add for inter blocks
@@ -12,13 +12,17 @@ intra (no MC, six coded blocks), each block of an inter macroblock is coded at p
          IDCT, intra blocks through the fused h263_intra dequantiser, inter blocks added
   mpeg4_gmc  MPEG-4 ASP S-VOPs with GMC (tests/mpv_gmc_cases.py): 2- and 3-point warps from random sprite trajectories, about 70 % of the
          macroblocks mcsel 16X16 (four in five of them skipped: no residual), the rest quarter-sample 16X16 and 4MV; residual as mpeg4
+  mpeg2_422  MPEG-2 4:2:2 (tests/mpv_ilace_cases.py), mixed like mpeg2; eight blocks per macroblock, field DCT in frame pictures moving
+         the chroma blocks too
+  mpeg4_ilace  interlaced MPEG-4 ASP: P and B pictures, quarter- and half-sample, about half of the macroblocks FIELD records (B-direct
+         ones among them), the rest 16X16 and 4MV; the Xvid IDCT with field DCT in half of the macroblocks
 The residual batches run without `clear`, so every timed flush transforms the same coefficients.  The arms `mc` (the motion compensation
 alone) and `flush` alternate within each round; a round times `steps` calls with CUDA events after `warmup` untimed ones.  Printed per
 batch and arm: the median and best ms per call, the spread (max - min) / median over the rounds, Mpixel/s of predicted pictures, and the
 algorithmic bytes over the median time as a fraction of the H100 SXM data sheet's 3.35 TB/s.  Bytes: per macroblock and direction 384 B
-of prediction read and 384 B written, plus the 44-byte record; per residual block 128 B of coefficients read and 64 B of pixels written
+of prediction read and 384 B written (4:2:2: 512 B each), plus the 44-byte record; per residual block 128 B of coefficients read and 64 B of pixels written
 (+ 64 B read for add, + 4 B of dequantiser record).  The CPU figure is the reference's own ff_mpv_motion (oracle/_ref/libmpvmcref.so,
-portable C; ref_mpvmc_gmc_picture of oracle/_ref/libmpvgmcref.so for the S-VOPs) over the same records on all host cores, one picture per thread (motion compensation
+portable C; ref_mpvmc_gmc_picture of oracle/_ref/libmpvgmcref.so for the S-VOPs, ref_mpvmc_cf_picture of libmpvcfref.so for 4:2:2) over the same records on all host cores, one picture per thread (motion compensation
 only).  After timing, every picture is
 rebuilt from its original bytes by one flush and compared with the chained checker: the reference's MC, then the IDCT and inverse
 quantiser oracles over the same batches.  The card's name, power limit and maximum SM clock come from a read-only nvidia-smi query and are
@@ -82,10 +86,45 @@ def gmc_batch(checker):
     return pics, [b for b in residual if len(b["off"])]
 
 
+def ilace_batch(kind, checker):
+    """sixteen MPEG-2 4:2:2 pictures or sixteen interlaced MPEG-4 pictures, with a decoder's residual"""
+    import mpv_ilace_cases as I
+    import mpv_mc_cases as M
+    pics = []
+    for i in range(16):
+        rng = np.random.default_rng(3000 + 100 * (kind == "mpeg4_ilace") + i)
+        if kind == "mpeg2_422":
+            st, ff, b = [(M.FRAME, 1, 0), (M.FRAME, 1, 1), (M.TOP, 1, 0), (M.BOTTOM, 0, 0)][i % 4]
+            pics.append(I.cf_picture(rng, 2, 120, 68, structure=st, first_field=ff, b=b, far=0.0, edge=0.02))
+        else:
+            pic = I.IlacePicture(rng, 120, 68, b=i & 1, no_rnd=(i >> 2) & 1, qpel=(i >> 1) & 1, width=1920, height=1080)
+            I.ilace_records(rng, pic, field=0.5, far=0.0, edge=0.02)
+            pics.append(pic)
+    return pics, I.residual(checker, pics, np.random.default_rng(11), xvid=kind == "mpeg4_ilace", clear=0)
+
+
+class _Ilace:
+    """the mpeg2_422 / mpeg4_ilace pictures' reference and checker (both the reference itself: tests/mpv_ilace_cases.py)"""
+
+    @staticmethod
+    def ref_lib():
+        import mpv_ilace_cases as I
+        return I.cf_ref_lib() if I.have_reference() else None
+
+    checker_lib = ref_lib
+
+    @staticmethod
+    def run_ref(lib, pic):
+        import mpv_ilace_cases as I
+        return I.run_ref(pic)
+
+
 def batch(kind, checker):
     import mpv_mc_cases as M
     if kind == "mpeg4_gmc":
         return gmc_batch(checker)
+    if kind in ("mpeg2_422", "mpeg4_ilace"):
+        return ilace_batch(kind, checker)
     pics = []
     for i in range(16):
         rng = np.random.default_rng(1000 * (kind == "mpeg4") + i)
@@ -111,21 +150,23 @@ def main():
     from libav_b200 import device
     from oracle import loader
     import mpv_gmc_cases as G
+    import mpv_ilace_cases as I
     import mpv_mc_cases as M
     L.init(0)
     checker = loader.ref() or loader.port()
     results = {"card": card()}
     print("card: %s" % results["card"])
-    for kind in ("mpeg2", "mpeg4", "mpeg4_gmc"):
-        C_ = G if kind == "mpeg4_gmc" else M          # the S-VOPs' reference, checker and device pictures
+    for kind in ("mpeg2", "mpeg4", "mpeg4_gmc", "mpeg2_422", "mpeg4_ilace"):
+        new_kind = kind in ("mpeg2_422", "mpeg4_ilace")
+        C_ = G if kind == "mpeg4_gmc" else _Ilace if new_kind else M          # the pictures' reference and checker
         ref, mc_checker = C_.ref_lib(), C_.checker_lib()
         pics, residual = batch(kind, checker)
-        g = G.GpuSvops(pics) if kind == "mpeg4_gmc" else M.GpuPictures(pics)
+        g = G.GpuSvops(pics) if kind == "mpeg4_gmc" else I.GpuPics(pics) if new_kind else M.GpuPictures(pics)
         res = M.GpuResidual(g, residual)
         work = res.work(g)
         n_mb_dir = sum(int(((p.recs["mv_dir"] & 1) != 0).sum() + ((p.recs["mv_dir"] & 2) != 0).sum()) for p in pics)
         n_rec = sum(len(p.recs) for p in pics)
-        mc_bytes = n_mb_dir * 768 + n_rec * 44
+        mc_bytes = n_mb_dir * (1024 if kind == "mpeg2_422" else 768) + n_rec * 44
         res_bytes = sum(len(b["off"]) * (192 + (64 if (b["mode"] == 1 and b["dq"] < 0) or b["dq"] in (1, 4, 6) else 0) + (4 if b["dq"] >= 0 else 0))
                         for b in residual)
         pixels = sum(16 * p.mb_rows * 16 * p.p["mb_width"] for p in pics)
