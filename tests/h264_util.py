@@ -74,8 +74,15 @@ def padded(plane, pad):
     return p, p[pad:-pad, pad:-pad]
 
 
+def _window(base, sy, sx, h, w):
+    """base[sy:sy + h, sx:sx + w], refusing a window the padding does not hold (a negative start would wrap around in numpy)"""
+    assert sy >= 0 and sx >= 0 and sy + h <= base.shape[0] and sx + w <= base.shape[1], "oracle_mc: pad too small for this vector"
+    return base[sy:sy + h, sx:sx + w]
+
+
 def oracle_mc(o, rec, refs, y, cb, cr, pad=48):
-    """refs: list of (y, cb, cr) planes; edge replication is emulated by padding the reference planes."""
+    """refs: list of (y, cb, cr) planes; edge replication is emulated by padding the reference planes by `pad` samples, which
+    must cover the farthest vector of `rec` (asserted per window)."""
     pr = []
     for (ry, rcb, rcr) in refs:
         pr.append((padded(ry, pad)[1], padded(rcb, pad)[1], padded(rcr, pad)[1]))
@@ -94,14 +101,14 @@ def oracle_mc(o, rec, refs, y, cb, cr, pad=48):
             win = np.zeros((n + 5, y.strides[0]), np.uint8)
             sy, sx = (my >> 2) + oy - 2, (mx >> 2) + ox - 2
             base = ry.base if ry.base is not None else ry
-            win[:, :n + 5] = base[sy + pad:sy + pad + n + 5, sx + pad:sx + pad + n + 5]
+            win[:, :n + 5] = _window(base, sy + pad, sx + pad, n + 5, n + 5)
             o.h264_qpel(avg, sizes[n], mc, dst, at(win, 2 * win.strides[0] + 2), y.strides[0])
         cw, chh = w // 2, h // 2
         for (pl, rp) in ((cb, rcb), (cr, rcr)):
             base = rp.base if rp.base is not None else rp
             sy, sx = (my >> 3), (mx >> 3)
             win = np.zeros((chh + 1, pl.strides[0]), np.uint8)
-            win[:, :cw + 1] = base[sy + pad:sy + pad + chh + 1, sx + pad:sx + pad + cw + 1]
+            win[:, :cw + 1] = _window(base, sy + pad, sx + pad, chh + 1, cw + 1)
             dst = at(pl, (int(r["y"]) // 2) * pl.strides[0] + int(r["x"]) // 2)
             o.h264_chroma(avg, {8: 0, 4: 1, 2: 2}[cw], dst, ptr(win), pl.strides[0], chh, mx & 7, my & 7)
 
