@@ -11,6 +11,7 @@
 #include "libavcodec/avcodec.h"
 #include "libavcodec/idctdsp.h"
 #include "libavcodec/fdctdsp.h"
+#include "libavcodec/faandct.h"
 #include "libavcodec/blockdsp.h"
 #include "libavcodec/me_cmp.h"
 #include "libavcodec/mpegvideodsp.h"
@@ -162,7 +163,7 @@ int ff_mpv_encode_init_cuda(MpegEncContext *s)
         .intra_ac_vlc_length = &s->intra_ac_vlc_length, .intra_ac_vlc_last_length = &s->intra_ac_vlc_last_length,
         .inter_ac_vlc_length = &s->inter_ac_vlc_length, .inter_ac_vlc_last_length = &s->inter_ac_vlc_last_length,
         .luma_dc_vlc_length = (const uint8_t *const *)&s->luma_dc_vlc_length,
-        .fdct = s->fdsp.fdct == ff_fdct_ifast ? 2 : s->fdsp.fdct == ff_jpeg_fdct_islow_8 ? 0 : -1,
+        .fdct = s->fdsp.fdct == ff_fdct_ifast ? 2 : s->fdsp.fdct == ff_jpeg_fdct_islow_8 ? 0 : s->fdsp.fdct == ff_faandct ? 6 : -1,
         .dequant = s->dct_unquantize_inter == s->dct_unquantize_h263_inter ? 3 :
                    s->dct_unquantize_inter == s->dct_unquantize_mpeg2_inter ? 1 + !!(s->avctx->flags & AV_CODEC_FLAG_BITEXACT) : 0,
         .idct_perm_none = s->idsp.perm_type == FF_IDCT_PERM_NONE,

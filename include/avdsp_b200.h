@@ -94,6 +94,13 @@ int ff_simple_idct10_batch_cuda(int mode, int16_t *blocks, uint8_t *frame, const
 int ff_xvid_idct_batch_cuda(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
                             size_t n, int tiles_per_row, int clear, void *stream);
 
+/* ff_faanidct / ff_faanidct_put / ff_faanidct_add (libavcodec/faanidct.c:113-159) over n blocks -- the IDCT of idct_algo FF_IDCT_FAAN.
+ * Arguments, addressing, modes, `clear` and alignment rules exactly as ff_xvid_idct_batch_cuda; put / add leave the coefficients untouched,
+ * mode 2 leaves the result (int16-truncated) in the blocks.  Bit-exact to the C code built without FMA: float passes whose products with
+ * the AAN constants are evaluated in double and rounded to float once per assignment (DESIGN.md section 5). */
+int ff_faanidct_batch_cuda(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
+                           size_t n, int tiles_per_row, int clear, void *stream);
+
 /* BlockDSPContext.clear_block / clear_blocks over n_blocks * 64 coefficients (blockdsp.c:29-37) and
  * fill_block_tab[w16 ? 0 : 1] over n records (blockdsp.c:39-58). */
 int ff_clear_blocks_batch_cuda(int16_t *blocks, size_t n_blocks, void *stream);
@@ -391,7 +398,7 @@ int ff_h264_flush_pictures_cuda(const FFH264PictureWork *work /* host struct */,
  *        6 nsse[sidx] (weight 8: the NULL-context default, me_cmp.c:331)   7 hadamard8_diff[4 + sidx] (intra)
  *        8 vsad[4 + sidx] (intra)   9 vsse[4 + sidx] (intra)   10 sum_abs_dctelem (cur_off in bytes into int16 blocks)
  *       11 dct_sad[sidx]   12 dct_max[sidx]   13 dct264_sad[sidx]   (me_cmp.c:538-621; for 11 / 12 `dxy` names the
- *          FDCTDSPContext.fdct the encoder context holds: 0 = ff_jpeg_fdct_islow_8, 2 = ff_fdct_ifast)
+ *          FDCTDSPContext.fdct the encoder context holds: 0 = ff_jpeg_fdct_islow_8, 2 = ff_fdct_ifast, 6 = ff_faandct)
  * These three only dereference the MpegEncContext's DSP tables, so the batch call covers them; their table slots are
  * left to the C code (a slot cannot know which fdct the caller's context selected).  quant_psnr, bit and rd
  * (me_cmp.c:621-782) need the quantiser and VLC length tables of a live encoder: see ff_me_cmp_enc_batch_cuda below. */
@@ -412,7 +419,7 @@ int ff_me_cmp_batch_cuda(int kind, int sidx, int dxy, const uint8_t *cur, const 
  *   out[i] = the slot's return value; last_index[i] (optional) = s->block_last_index[0] as the C function leaves it.
  * A DC level outside the DC table (|level| > 255: impossible for 8-bit differences with dc_scale >= 1) is clamped to its ends. */
 typedef struct FFMECmpEncState {
-    int32_t fdct;                  /* s->fdsp.fdct: 0 ff_jpeg_fdct_islow_8, 2 ff_fdct_ifast */
+    int32_t fdct;                  /* s->fdsp.fdct: 0 ff_jpeg_fdct_islow_8, 2 ff_fdct_ifast, 6 ff_faandct */
     int32_t dequant;               /* s->dct_unquantize_intra / _inter (mpegvideo_enc.c:1613-1622): 0 mpeg1, 1 mpeg2, 2 mpeg2 under
                                       AV_CODEC_FLAG_BITEXACT (mismatch control on intra blocks too), 3 h263 */
     int32_t qscale, mb_intra, y_dc_scale, h263_aic;
@@ -442,7 +449,7 @@ int ff_me_cmp_enc_batch_cuda(int kind, int sidx, const void *enc_state, const ui
  * quant_psnr / bit / rd metrics; luma_dc_vlc_length is not read and may be NULL).  Under ff_fdct_ifast the trellis weighs its distortion with
  * ff_inv_aanscales, which the library derives from its definition (round(4096 / (a(u) a(v))), a(0) = 1, a(k) = sqrt(2) cos(k pi / 16)). */
 typedef struct FFMpvQuantState {
-    int32_t fdct;                                   /* s->fdsp.fdct: 0 ff_jpeg_fdct_islow_8, 2 ff_fdct_ifast */
+    int32_t fdct;                                   /* s->fdsp.fdct: 0 ff_jpeg_fdct_islow_8, 2 ff_fdct_ifast, 6 ff_faandct */
     int32_t out_format;                             /* enum OutputFormat (mpegutils.h): 0 FMT_MPEG1, 1 FMT_H261, 2 FMT_H263, 3 FMT_MJPEG */
     int32_t mpeg_quant, h263_aic;
     int32_t intra_quant_bias, inter_quant_bias;     /* QUANT_BIAS_SHIFT units; the trellis ignores them (its own thresholds) */
@@ -465,7 +472,7 @@ typedef struct FFMpvNoiseReduction {                /* DEVICE pointers: s->dct_o
     int32_t *dct_error_sum, *dct_count;
 } FFMpvNoiseReduction;
 /* device-resident copy of a state (one per picture, or per change of matrices); NULL + avb200_last_error() for a bad state: an fdct other
- * than 0 or 2, an out_format outside 0..3, a scantable that is not a permutation starting at 0.  vlc may be NULL when no call uses trellis. */
+ * than 0, 2 or 6, an out_format outside 0..3, a scantable that is not a permutation starting at 0.  vlc may be NULL when no call uses trellis. */
 void *ff_mpv_quant_state_cuda(const FFMpvQuantState *state, const FFMECmpVlcTables *vlc);
 void ff_mpv_quant_state_free_cuda(void *quant_state);
 /* n blocks, one thread each, on `stream` without synchronising.  Input: s1 == NULL -> blocks[i] already holds what get_pixels /
@@ -587,6 +594,12 @@ typedef struct FFMpvMCPicture {
     int sprite_offset[2][2], sprite_delta[2][2];
     int interlaced;                     /* !s->progressive_sequence, read in out_format 2 only: FIELD records of the frame picture are taken */
 } FFMpvMCPicture;
+/* put_dct / add_dequant_dct (mpegvideo.c:1401-1427) with the FAAN IDCT: same arguments, kinds, skipping rules and alignment rules as
+ * ff_mpeg_dequant_xvid_idct_batch_cuda, the transform of ff_faanidct_batch_cuda. */
+int ff_mpeg_dequant_faanidct_batch_cuda(int kind, const FFMpegDequantTables *tables, const FFMpegDequantBlock *recs, int16_t *blocks,
+                                        uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row,
+                                        int clear, void *stream);
+
 int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, int n_pictures, uint32_t *rejected, void *stream);
 
 /* The flush point of an mpegvideo decoder back-end: the decoder parses a batch of pictures, records the motion of every inter macroblock
@@ -595,6 +608,7 @@ int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, in
  * point -- the simple or the Xvid transform, with no inverse quantiser or one of the seven kinds of ff_mpeg_dequant_idct_batch_cuda:
  *   dequant -1, transform 0: ff_simple_idct_batch_cuda(mode, ...)        dequant k, transform 0: ff_mpeg_dequant_idct_batch_cuda(k, ...)
  *   dequant -1, transform 1: ff_xvid_idct_batch_cuda(mode, ...)          dequant k, transform 1: ff_mpeg_dequant_xvid_idct_batch_cuda(k, ...)
+ *   dequant -1, transform 3: ff_faanidct_batch_cuda(mode, ...)           dequant k, transform 3: ff_mpeg_dequant_faanidct_batch_cuda(k, ...)
  * Intra blocks (idct_put / put_dct) and inter blocks (idct_add / add_dct / add_dequant_dct) go in separate batches, and so do frame and
  * field DCT blocks: a field-DCT block of a macroblock at dest has dct_linesize = 2 * linesize and its lower blocks start one line down
  * (mpegvideo.c:1534-1535).  Blocks are addressed through dst_off (byte offsets into `frame`).  Every batch is checked before anything is
@@ -602,7 +616,7 @@ int ff_mpv_motion_batch_cuda(const FFMpvMCPicture *pictures /* host array */, in
  * the flush with -1 after the stages before it were enqueued.  Then, when loop_filter is set, the H.263 deblocking filter of those pictures
  * (ff_h263_loop_filter_batch_cuda), checked with everything else before the first stage is enqueued. */
 typedef struct FFMpvResidualBatch {
-    int transform;                       /* 0 simple IDCT, 1 Xvid IDCT */
+    int transform;                       /* 0 simple IDCT, 1 Xvid IDCT, 3 FAAN IDCT (2 is not a transform) */
     int dequant;                         /* -1: the blocks are dequantised already; 0..6: the inverse quantiser kind fused in front */
     int mode;                            /* dequant -1: 0 put, 1 add (a fused kind puts for intra kinds, adds for inter kinds) */
     const FFMpegDequantTables *tables;   /* host struct, dequant >= 0 */
@@ -645,12 +659,13 @@ int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *work /* host struct */, v
 
 /* FDCTDSPContext (libavcodec/fdctdsp.h:26-29), in place over n blocks: which 0 = ff_jpeg_fdct_islow_8, 1 =
  * ff_fdct248_islow_8 (jfdctint_template.c:260-398), 2 = ff_fdct_ifast, 3 = ff_fdct_ifast248 (jfdctfst.c:207-332), 4 = ff_jpeg_fdct_islow_10,
- * 5 = ff_fdct248_islow_10 (the BIT_DEPTH 10 instances: PASS1_BITS 1, OUT_SHIFT 2; thread per block, untuned). */
+ * 5 = ff_fdct248_islow_10 (the BIT_DEPTH 10 instances: PASS1_BITS 1, OUT_SHIFT 2; thread per block, untuned), 6 = ff_faandct, 7 = ff_faandct248
+ * (libavcodec/faandct.c, bit-exact: float passes with the C code's double products; thread per block, untuned). */
 int ff_fdct_batch_cuda(int which, int16_t *blocks, size_t n, void *stream);
 /* PixblockDSPContext.get_pixels / diff_pixels (libavcodec/pixblockdsp_template.c:24-66) over n 8x8 blocks, optionally
  * followed by the forward DCT in the same kernel -- the encoder's "fetch (difference) -> fdct" front end
  * (mpegvideo_enc.c:1923-2019 dct loop).  Block i reads s1 + off1[i] and, if s2 != NULL, subtracts s2 + off2[i] (off2
- * NULL = the same offsets); which_fdct < 0 stores the samples / differences, 0..3 select the transform as in
+ * NULL = the same offsets); which_fdct < 0 stores the samples / differences, 0..3, 6 and 7 select the transform as in
  * ff_fdct_batch_cuda.  Output: int16 blocks[n][64], row-major. */
 int ff_pixblock_fdct_batch_cuda(int which_fdct, const uint8_t *s1, const uint8_t *s2, const uint32_t *off1, const uint32_t *off2,
                                 ptrdiff_t stride, int16_t *blocks, size_t n, void *stream);
@@ -726,8 +741,8 @@ int  sws_debug_slot_view_cuda(int srcW, int srcH, int srcFormat, int dstW, int d
 /* One more arch behind ff_idctdsp_init()'s dispatch (libavcodec/idctdsp.c:183-188; same shape as
  * ff_idctdsp_init_x86, libavcodec/idctdsp.h:109-110).  AVCodecContext is opaque to this library, so the
  * two fields the hook needs are passed by value (INTEGRATION.md shows the one-line caller).
- * Taken over: idct_algo FF_IDCT_SIMPLE / FF_IDCT_AUTO at 8 bit, and bits_per_raw_sample 10 (ff_simple_idct_*_10 whatever idct_algo says,
- * idctdsp.c:151-155); anything else leaves `c` untouched. */
+ * Taken over: idct_algo FF_IDCT_SIMPLE / FF_IDCT_AUTO and FF_IDCT_FAAN (AVB_FF_IDCT_FAAN: ff_faanidct*, FF_IDCT_PERM_NONE) at 8 bit, and
+ * bits_per_raw_sample 10 (ff_simple_idct_*_10 whatever idct_algo says, idctdsp.c:151-155); anything else leaves `c` untouched. */
 void ff_idctdsp_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample, unsigned high_bit_depth);
 /* The arch hook of ff_xvid_idct_init (libavcodec/xvididct.c:333-350), called after it: idct / idct_put / idct_add, perm_type =
  * FF_IDCT_PERM_NONE and an identity idct_permutation when bits_per_raw_sample <= 8 and idct_algo is FF_IDCT_AUTO or FF_IDCT_XVID
@@ -735,7 +750,8 @@ void ff_idctdsp_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sam
 void ff_xvid_idct_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample);
 void ff_blockdsp_init_cuda(BlockDSPContext *c);   /* libavcodec/blockdsp.c:60-74 */
 /* libavcodec/fdctdsp.c:27-50 (same shape as ff_fdctdsp_init_x86): dct_algo FF_DCT_AUTO / FF_DCT_INT -> islow,
- * FF_DCT_FASTINT -> ifast; bits_per_raw_sample 10 -> jpeg_fdct_islow_10 / fdct248_islow_10; FF_DCT_FAAN is left to the C path */
+ * FF_DCT_FASTINT -> ifast, FF_DCT_FAAN -> ff_faandct / ff_faandct248; bits_per_raw_sample 10 -> jpeg_fdct_islow_10 / fdct248_islow_10
+ * whatever dct_algo says */
 void ff_fdctdsp_init_cuda(FDCTDSPContext *c, int dct_algo, int bits_per_raw_sample, unsigned high_bit_depth);
 /* libavcodec/me_cmp.c:895-944: every slot ff_me_cmp_init fills except the encoder-state metrics */
 void ff_me_cmp_init_cuda(MECmpContext *c);
@@ -761,8 +777,8 @@ void ff_me_cmp_enc_uninit_cuda(struct MpegEncContext *s);
  * *view->fast_dct_quantize with the plain slot and *view->dct_quantize with the trellis slot when `trellis` (avctx->trellis) is set, the
  * plain one otherwise.  The slots have the reference's signature and apply noise reduction themselves when *view->dct_error_sum is set, as the
  * C quantisers do.  Like the metric slots they read the live context through `view` on every call (one block: stage, copy, kernel, copy
- * back, synchronise).  Returns 0, or -1 with the context untouched for: a permuting IDCT, an fdct other than islow / ifast (FF_DCT_FAAN,
- * a 10-bit encoder), quantizer_noise_shaping, slice threading (slice_context_count > 1), a NULL view pointer.  Slice threading is refused
+ * back, synchronise).  Returns 0, or -1 with the context untouched for: a permuting IDCT, an fdct other than islow / ifast / FAAN (a
+ * 10-bit encoder), quantizer_noise_shaping, slice threading (slice_context_count > 1), a NULL view pointer.  Slice threading is refused
  * because the view points into the one context it was made from: ff_update_duplicate_context copies the slots into the per-thread
  * contexts, whose mb_intra, lambda2, coded_score and noise-reduction sums are their own.  Such an encoder keeps the C quantisers (the
  * batched call serves it instead).  Call it after ff_me_cmp_enc_init_cuda, which must still see

@@ -38,6 +38,7 @@ typedef struct IDCTDSPContext {
 #define AVB_FF_IDCT_AUTO   0
 #define AVB_FF_IDCT_SIMPLE 2
 #define AVB_FF_IDCT_XVID   14
+#define AVB_FF_IDCT_FAAN   20
 
 /* ---- libavcodec/fdctdsp.h:26-29 ---- */
 typedef struct FDCTDSPContext {
@@ -47,6 +48,7 @@ typedef struct FDCTDSPContext {
 #define AVB_FF_DCT_AUTO    0
 #define AVB_FF_DCT_FASTINT 1
 #define AVB_FF_DCT_INT     2
+#define AVB_FF_DCT_FAAN    6
 
 /* ---- libavcodec/blockdsp.h:29-37 ---- */
 typedef void (*op_fill_func)(uint8_t *block, uint8_t value, ptrdiff_t line_size, int h);

@@ -59,6 +59,7 @@ PROTOTYPES = {
     "ff_simple_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_simple_idct10_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, vp]),
     "ff_xvid_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
+    "ff_faanidct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_pixels_clamped_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, vp]),
     "ff_clear_blocks_batch_cuda": (i32, [vp, sz, vp]),
     "ff_fill_blocks_batch_cuda": (i32, [vp, vp, vp, pd, i32, i32, sz, vp]),
@@ -78,6 +79,7 @@ PROTOTYPES = {
     "ff_mpeg_dequant_batch_cuda": (i32, [i32, vp, vp, vp, sz, vp]),
     "ff_mpeg_dequant_idct_batch_cuda": (i32, [i32, vp, vp, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_mpeg_dequant_xvid_idct_batch_cuda": (i32, [i32, vp, vp, vp, vp, vp, pd, sz, i32, i32, vp]),
+    "ff_mpeg_dequant_faanidct_batch_cuda": (i32, [i32, vp, vp, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_me_cmp_batch_cuda": (i32, [i32, i32, i32, vp, vp, pd, i32, vp, sz, vp, vp]),
     "ff_h264_idct_add_mb_batch_hbd_cuda": (i32, [i32, i32, vp, sz, vp, sz, vp, vp, vp, vp, i32, i32, vp]),
     "ff_h264_mc_batch_hbd_cuda": (i32, [i32, i32, vp, sz, vp, vp, vp, vp, i32, i32, i32, i32, vp]),

@@ -17,6 +17,8 @@ int launch_mpeg_dequant_idct(int kind, const DqTables &t, const uint32_t *recs, 
                              const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st);
 int launch_mpeg_dequant_xvid_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
                                   const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st);
+int launch_mpeg_dequant_faan_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
+                                  const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st);
 int launch_fill_blocks(uint8_t *frame, const uint32_t *dst_off, const uint8_t *value, ptrdiff_t stride, int h,
                        int w16, size_t n, cudaStream_t st);
 }
@@ -79,6 +81,20 @@ int ff_mpeg_dequant_xvid_idct_batch_cuda(int kind, const FFMpegDequantTables *t,
         return -1;
     }
     return launch_mpeg_dequant_xvid_idct(kind, d, reinterpret_cast<const uint32_t *>(recs), blocks, frame, dst_off, stride, n, tiles_per_row,
+                                         clear, (cudaStream_t)stream);
+}
+int ff_mpeg_dequant_faanidct_batch_cuda(int kind, const FFMpegDequantTables *t, const FFMpegDequantBlock *recs, int16_t *blocks,
+                                        uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row,
+                                        int clear, void *stream)
+{
+    avb::enter();
+    DqTables d;
+    if (dq_tables("ff_mpeg_dequant_faanidct_batch_cuda", kind, t, d)) return -1;
+    if (n && (((uintptr_t)blocks & 15) || (((uintptr_t)frame | (uintptr_t)stride) & 7))) {
+        set_error_msg("ff_mpeg_dequant_faanidct_batch_cuda", "blocks must be 16-byte aligned, frame and stride multiples of 8");
+        return -1;
+    }
+    return launch_mpeg_dequant_faan_idct(kind, d, reinterpret_cast<const uint32_t *>(recs), blocks, frame, dst_off, stride, n, tiles_per_row,
                                          clear, (cudaStream_t)stream);
 }
 int ff_clear_blocks_batch_cuda(int16_t *blocks, size_t n_blocks, void *stream)
@@ -237,6 +253,7 @@ void slot_fill8(uint8_t *b, uint8_t v, ptrdiff_t ls, int h) { slot_fill(b, v, ls
 }  // namespace
 
 namespace avb { void idct10_install(IDCTDSPContext *c); }      // idct10.cu
+namespace avb { void faan_idct_install(IDCTDSPContext *c); }   // faan_idct.cu
 
 extern "C" {
 
@@ -262,6 +279,8 @@ void ff_idctdsp_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sam
         // ff_idctdsp_init() calls ff_init_scantable_permutation() after the arch hooks; keep the table
         // consistent for callers that invoke the hook on its own.
         for (int i = 0; i < 64; i++) c->idct_permutation[i] = (uint8_t)i;
+    } else if (idct_algo == AVB_FF_IDCT_FAAN) {
+        faan_idct_install(c);                      // idctdsp.c:162-166
     }
 }
 

@@ -4,9 +4,11 @@
 //                     columns <-4, 17>
 //   col_248<FAST>     the column pass of the 2-4-8 variants (jfdctint_template.c:340-398, jfdctfst.c:234-332)
 //   ifast_1d          ff_fdct_ifast (libavcodec/jfdctfst.c:141-232), both passes
+//   faan::*           ff_faandct / ff_faandct248 (libavcodec/faandct.c), faan_dct.cuh
 // Thread-local arithmetic only (also compiled by tests/hostsim/).
 #pragma once
 #include "common.cuh"
+#include "faan_dct.cuh"
 
 namespace avb {
 
@@ -61,12 +63,20 @@ __device__ __forceinline__ void ifast_1d(const int (&in)[8], int (&out)[8])
     out[5] = z13 + z2; out[3] = z13 - z2; out[1] = z11 + z4; out[7] = z11 - z4;
 }
 
-// The two passes of the 2-D forward DCT as FDCTDSPContext.fdct runs them on an int16 block (FDCT as in ff_fdct_batch_cuda 0..3):
+// The two passes of the 2-D forward DCT as FDCTDSPContext.fdct runs them on an int16 block (FDCT as in ff_fdct_batch_cuda 0..3, 6, 7):
 // fdct_row = the row pass of one row with the int16 write-back the C code does between the passes, fdct_cols = the column pass over a
-// block held in registers (not yet truncated: the caller's int16 store does that).
+// block held in registers (not yet truncated: the caller's int16 store does that).  The FAAN transforms (6 ff_faandct, 7 ff_faandct248)
+// keep float between the passes (faandct.c's temp[]): their row pass leaves the float's bits in m, and their column pass reads them back.
 template <int FDCT>
 __device__ __forceinline__ void fdct_row(const int (&in)[8], int (&out)[8])
 {
+    if constexpr (FDCT >= 6) {
+        float t[8];
+        faan::fdct_row(in, t);
+#pragma unroll
+        for (int k = 0; k < 8; k++) out[k] = __float_as_int(t[k]);
+        return;
+    }
     int o[8];
     if (FDCT < 2) islow_1d<4, 9>(in, o); else ifast_1d(in, o);
 #pragma unroll
@@ -80,7 +90,13 @@ __device__ __forceinline__ void fdct_cols(int (&m)[8][8])
         int in[8], o[8];
 #pragma unroll
         for (int k = 0; k < 8; k++) in[k] = m[k][c];
-        if (FDCT == 0) islow_1d<-4, 17>(in, o);
+        if constexpr (FDCT >= 6) {
+            float t[8];
+#pragma unroll
+            for (int k = 0; k < 8; k++) t[k] = __int_as_float(in[k]);
+            if (FDCT == 6) faan::fdct_col(t, c, o); else faan::fdct248_col(t, c, o);
+        }
+        else if (FDCT == 0) islow_1d<-4, 17>(in, o);
         else if (FDCT == 1) col_248<false>(in, o);
         else if (FDCT == 2) ifast_1d(in, o);
         else col_248<true>(in, o);
@@ -90,7 +106,7 @@ __device__ __forceinline__ void fdct_cols(int (&m)[8][8])
 }
 
 // PixblockDSPContext.get_pixels / diff_pixels (pixblockdsp_template.c:24-66) of the 8x8 block at a (minus the one at b, b != NULL),
-// optionally followed by the forward DCT in the same thread (FDCT as in ff_fdct_batch_cuda 0..3; < 0: the samples / differences): the
+// optionally followed by the forward DCT in the same thread (FDCT as in ff_fdct_batch_cuda 0..3, 6, 7; < 0: the samples / differences): the
 // spatial block never exists as int16 in memory.  m holds what the C code leaves in its int16 block (the column pass is not yet truncated).
 // Shared by pixblock_kernel (me_cmp.cu) and the quantiser's front end (mpv_quant.cu).
 template <int FDCT>

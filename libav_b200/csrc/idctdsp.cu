@@ -16,12 +16,15 @@
 // Two tiles per warp are double-buffered so the next group's loads fly during the math.
 // Algorithmic traffic: put 128 B in + 64 B out (+4 B offset) per block; add 256 B; idct 256 B.
 // The two passes are a policy of the kernel template (SimpleIdct here, XvidIdct in xvid_idct.cuh for ff_xvid_idct): everything else
-// -- staging, fetch, addressing, fused clear and dequantisation -- is shared.
+// -- staging, fetch, addressing, fused clear and dequantisation -- is shared.  The FAAN IDCT (float between the passes) has a kernel body of
+// its own, faan_idct_kernel, over the same staging and inverse quantisers.
 #include "common.cuh"
 #include <type_traits>
 #include <cuda.h>            // CUtensorMap only; the encoder is looked up at run time (no libcuda link dependency)
 #include "idct_dq.h"
 #include "xvid_idct.cuh"
+#include "faan_dct.cuh"
+#include "block_stage.cuh"
 
 namespace avb {
 
@@ -357,6 +360,89 @@ simple_idct_kernel(int16_t *__restrict__ blocks, uint8_t *__restrict__ frame,
     }
 }
 
+// The FAAN IDCT (ff_faanidct / _put / _add, faan_dct.cuh) over the same staging: its data between the passes is float, so it has its own
+// body rather than a transform policy of simple_idct_kernel.  One thread per block; the lane's eight rows arrive as LDS.128 from the
+// warp's swizzled tile (WarpBlockStage), both passes run in registers.  MODE 0 put, 1 add, 2 in place (the result goes back through the
+// tile and leaves as coalesced 512-byte stores); CLEAR zeroes a put / add block afterwards; DQ != 0 fuses inverse quantiser kind DQ - 1
+// in front, with the skipping rule of simple_idct_kernel.  put / add leave the coefficients untouched, as the C functions do.
+template <int MODE, bool CLEAR, int DQ = 0>
+__global__ void __launch_bounds__(IDCT_WARPS * 32)
+faan_idct_kernel(int16_t *__restrict__ blocks, uint8_t *__restrict__ frame, const uint32_t *__restrict__ dst_off, ptrdiff_t stride, size_t n,
+                 int tiles_per_row, const typename std::conditional<DQ != 0, DqArgs, NoDq>::type dq = {})
+{
+    __shared__ __align__(128) uint4 tile[IDCT_WARPS][2][256];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const WarpBlockStage S(&tile[warp][0][0], lane);
+    const size_t groups = (n + 31) / 32, gstride = (size_t)gridDim.x * IDCT_WARPS;
+    size_t g = (size_t)blockIdx.x * IDCT_WARPS + warp;
+    unsigned buf = 0;
+    if (g < groups) S.issue(blocks, g, n, S.buffer(0));
+    for (; g < groups; g += gstride, buf ^= 4096u) {
+        const size_t gn = g + gstride;
+        const unsigned tb = S.buffer(buf);
+        if (gn < groups) { S.issue(blocks, gn, n, S.buffer(buf ^ 4096u)); cp_async_wait<1>(); } else cp_async_wait<0>();
+        __syncwarp();
+        const size_t i = g * 32 + lane;
+        bool live = i < n;
+        float t[8][8];
+        [[maybe_unused]] uint32_t rec = 0;
+        [[maybe_unused]] DqLane L = {};
+        [[maybe_unused]] int sum = -1;
+        if constexpr (DQ != 0) {
+            rec = live ? dq.recs[i] : 0;
+            L = dq_lane<DQ - 1>(rec, dq.t);
+            if (MODE == 1 && (int8_t)(rec >> 8) < 0) live = false;
+        }
+#pragma unroll
+        for (int r = 0; r < 8; r++) {
+            uint4 w = S.row(tb, r);
+            if constexpr (DQ != 0) w = dq_row<DQ - 1>(w, r, dq.t, L, sum);
+            const int x[8] = { lo16s(w.x), hi16s(w.x), lo16s(w.y), hi16s(w.y), lo16s(w.z), hi16s(w.z), lo16s(w.w), hi16s(w.w) };
+            faan::idct_row(x, r, t[r]);
+        }
+#pragma unroll
+        for (int c = 0; c < 8; c++) {
+            float col[8];
+#pragma unroll
+            for (int k = 0; k < 8; k++) col[k] = t[k][c];
+            faan::idct_1d(col);
+#pragma unroll
+            for (int k = 0; k < 8; k++) t[k][c] = col[k];
+        }
+        if (MODE == 2) {
+            __syncwarp();                                    // every lane has read its rows: the tile takes the results
+#pragma unroll
+            for (int y = 0; y < 8; y++) {
+                int v[8];
+#pragma unroll
+                for (int c = 0; c < 8; c++) v[c] = __float2int_rn(t[y][c]);
+                S.put_row(tb, y, make_uint4(pack16(v[0], v[1]), pack16(v[2], v[3]), pack16(v[4], v[5]), pack16(v[6], v[7])));
+            }
+            S.flush(blocks, g, n, tb);
+        } else if (live) {
+            uint8_t *dst = frame + block_dst(dst_off, i, tiles_per_row, stride);
+#pragma unroll
+            for (int y = 0; y < 8; y++) {
+                int v[8];
+#pragma unroll
+                for (int c = 0; c < 8; c++) v[c] = __float2int_rn(t[y][c]);
+                if (MODE == 1) {
+                    const uint2 p = *reinterpret_cast<const uint2 *>(dst + y * stride);
+#pragma unroll
+                    for (int k = 0; k < 4; k++) { v[k] += byte_of(p.x, k); v[4 + k] += byte_of(p.y, k); }
+                }
+                *reinterpret_cast<uint2 *>(dst + y * stride) = make_uint2(pack4_sat_u8(v[0], v[1], v[2], v[3]), pack4_sat_u8(v[4], v[5], v[6], v[7]));
+            }
+            if (CLEAR) {
+                uint4 *b = reinterpret_cast<uint4 *>(blocks) + i * 8;
+#pragma unroll
+                for (int y = 0; y < 8; y++) b[y] = make_uint4(0, 0, 0, 0);
+            }
+        }
+        __syncwarp();                                        // this buffer is free for the load issued next iteration
+    }
+}
+
 // put / put_signed / add pixels clamped (idctdsp.c:85-145): 16-byte row in, 8-byte row out.
 // One thread per block row; a warp covers 4 blocks.  Purely HBM bound.
 template <int MODE>
@@ -546,6 +632,45 @@ int launch_mpeg_dequant_xvid_idct(int kind, const DqTables &t, const uint32_t *r
                                   const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st)
 {
     return launch_dequant_idct8<XvidIdct>("mpeg_dequant_xvid_idct_batch", kind, t, recs, blocks, frame, dst_off, stride, n, tiles_per_row, clear, st);
+}
+
+// the staged FAAN IDCT: 16-byte aligned blocks and, for put / add, 8-byte aligned destinations (faan_idct.cu decides)
+int launch_faan_idct_staged(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride,
+                            size_t n, int tiles_per_row, int clear, cudaStream_t st)
+{
+    if (n == 0) return 0;
+    const int grid = grid_for((n + 31) / 32, IDCT_WARPS, 16);
+    const dim3 b(IDCT_WARPS * 32);
+    if (mode == 0) {
+        if (clear) faan_idct_kernel<0, true><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        else       faan_idct_kernel<0, false><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+    } else if (mode == 1) {
+        if (clear) faan_idct_kernel<1, true><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+        else       faan_idct_kernel<1, false><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+    } else {
+        faan_idct_kernel<2, false><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row);
+    }
+    return check_launch("faanidct_batch");
+}
+
+int launch_mpeg_dequant_faan_idct(int kind, const DqTables &t, const uint32_t *recs, int16_t *blocks, uint8_t *frame,
+                                  const uint32_t *dst_off, ptrdiff_t stride, size_t n, int tiles_per_row, int clear, cudaStream_t st)
+{
+    static const char *who = "mpeg_dequant_faanidct_batch";
+    if (n == 0) return 0;
+    if (!dst_off && tiles_per_row <= 0) { set_error_msg(who, "need dst_off or tiles_per_row"); return -1; }
+    const int grid = grid_for((n + 31) / 32, IDCT_WARPS, 16);
+    const dim3 b(IDCT_WARPS * 32);
+    DqArgs a; a.recs = recs; a.t = t;
+#define AVB_DQ(K, MODE) \
+    case K: if (clear) faan_idct_kernel<MODE, true, K + 1><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, a); \
+            else       faan_idct_kernel<MODE, false, K + 1><<<grid, b, 0, st>>>(blocks, frame, dst_off, stride, n, tiles_per_row, a); break;
+    switch (kind) {
+    AVB_DQ(0, 0) AVB_DQ(1, 1) AVB_DQ(2, 0) AVB_DQ(3, 0) AVB_DQ(4, 1) AVB_DQ(5, 0) AVB_DQ(6, 1)
+    default: set_error_msg(who, "bad kind"); return -1;
+    }
+#undef AVB_DQ
+    return check_launch(who);
 }
 
 int launch_pixels_clamped(int mode, const int16_t *blocks, uint8_t *frame, const uint32_t *dst_off,

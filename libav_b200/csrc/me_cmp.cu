@@ -15,6 +15,7 @@
 #include "../../include/avdsp_b200.h"
 
 namespace avb { int fdct10_launch(int which, int16_t *blocks, size_t n, cudaStream_t st); }      // fdct10.cu
+namespace avb { int faan_fdct_launch(int which, int16_t *blocks, size_t n, cudaStream_t st); }   // faan_idct.cu
 
 namespace avb {
 
@@ -324,7 +325,7 @@ mpeg4_qpel_kernel(const FFQpelRecord *__restrict__ recs, size_t n, uint8_t *__re
 }
 
 // Encoder-state metrics that only need the DSP tables (me_cmp.c:538-621): kind 11 dct_sad, 12 dct_max (diff_pixels ->
-// FDCTDSPContext.fdct -> sum / max of |coefficient|; dxy selects the transform: 0 islow, 2 ifast), 13 dct264_sad (diff ->
+// FDCTDSPContext.fdct -> sum / max of |coefficient|; dxy selects the transform: 6 FAAN, 2 ifast, any other islow), 13 dct264_sad (diff ->
 // H.264 8x8 forward transform rows then columns -> sum of |result|).  Warp per record, one lane per 8x8 quadrant.
 __device__ __forceinline__ void dct264_1d(const int (&v)[8], int (&o)[8])
 {
@@ -337,10 +338,17 @@ __device__ __forceinline__ void dct264_1d(const int (&v)[8], int (&o)[8])
     o[4] = a0 - a1; o[5] = a6 - (a5 >> 2); o[6] = (a2 >> 1) - a3; o[7] = (a4 >> 2) - a7;
 }
 
-template <int T>   // T 0 islow, 2 ifast, 4 h264
+template <int T>   // T 0 islow, 2 ifast, 4 h264, 6 FAAN (ff_faandct)
 __device__ __forceinline__ int dct_metric_block(const uint8_t *a, const uint8_t *b, ptrdiff_t st, bool want_max)
 {
     int m[8][8];
+    if constexpr (T == 6) {
+        pixblock_fetch<6>(a, b, st, m);
+        int s = 0;
+#pragma unroll
+        for (int k = 0; k < 64; k++) { const int v = (int)(int16_t)m[k >> 3][k & 7]; s = want_max ? max(s, iabs_m(v)) : s + iabs_m(v); }
+        return s;
+    }
 #pragma unroll
     for (int r = 0; r < 8; r++) {
         int in[8], o[8];
@@ -376,6 +384,7 @@ me_cmp_dct_kernel(int kind, int sidx, int fdct_sel, const uint8_t *__restrict__ 
         const uint8_t *a = cur + recs[ri].cur_off + (lane & 1) * 8 + (lane >> 1) * 8 * st, *b = ref + recs[ri].ref_off + (lane & 1) * 8 + (lane >> 1) * 8 * st;
         if (kind == 13) s = dct_metric_block<4>(a, b, st, false);
         else if (fdct_sel == 2) s = dct_metric_block<2>(a, b, st, kind == 12);
+        else if (fdct_sel == 6) s = dct_metric_block<6>(a, b, st, kind == 12);
         else s = dct_metric_block<0>(a, b, st, kind == 12);
     }
     s = warp_sum(s);
@@ -435,6 +444,7 @@ int ff_fdct_batch_cuda(int which, int16_t *blocks, size_t n, void *stream)
     case 2: fdct_kernel<2><<<grid, 128, 0, st>>>(blocks, n); break;
     case 3: fdct_kernel<3><<<grid, 128, 0, st>>>(blocks, n); break;
     case 4: case 5: return fdct10_launch(which, blocks, n, st);          // the 10-bit instances, fdct10.cu
+    case 6: case 7: return avb::faan_fdct_launch(which, blocks, n, st);   // ff_faandct / ff_faandct248, faan_idct.cu
     default: set_error_msg("fdct_batch", "bad transform selector"); return -1;
     }
     return check_launch("fdct_batch");
@@ -461,6 +471,8 @@ int ff_pixblock_fdct_batch_cuda(int which_fdct, const uint8_t *s1, const uint8_t
     case 1: pixblock_kernel<1><<<grid, 128, 0, st>>>(s1, s2, off1, off2, stride, blocks, n); break;
     case 2: pixblock_kernel<2><<<grid, 128, 0, st>>>(s1, s2, off1, off2, stride, blocks, n); break;
     case 3: pixblock_kernel<3><<<grid, 128, 0, st>>>(s1, s2, off1, off2, stride, blocks, n); break;
+    case 6: pixblock_kernel<6><<<grid, 128, 0, st>>>(s1, s2, off1, off2, stride, blocks, n); break;
+    case 7: pixblock_kernel<7><<<grid, 128, 0, st>>>(s1, s2, off1, off2, stride, blocks, n); break;
     default:
         if (which_fdct >= 0) { set_error_msg("pixblock_fdct_batch", "bad transform selector"); return -1; }
         pixblock_kernel<-1><<<grid, 128, 0, st>>>(s1, s2, off1, off2, stride, blocks, n); break;

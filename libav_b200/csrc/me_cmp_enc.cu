@@ -112,9 +112,21 @@ __device__ inline void enc_idct_col(const int16_t *c, int (&out)[8])
     out[2] = (int)(e2 + o2) >> 20; out[5] = (int)(e2 - o2) >> 20; out[3] = (int)(e3 + o3) >> 20; out[4] = (int)(e3 - o3) >> 20;
 }
 
-// s->fdsp.fdct on an int16 block held by the thread (int16 write-back between the passes, like fdct_kernel)
-__device__ inline void enc_fdct(int16_t *b, bool fast)
+// s->fdsp.fdct on an int16 block held by the thread (int16 write-back between the passes, like fdct_kernel); fdct as in FFMECmpEncState
+__device__ inline void enc_fdct(int16_t *b, int fdct)
 {
+    if (fdct == 6) {                                              // ff_faandct: float between the passes (fdct_dev.cuh)
+        int m[8][8];
+        for (int r = 0; r < 8; r++) {
+            int in[8];
+            for (int k = 0; k < 8; k++) in[k] = b[8 * r + k];
+            fdct_row<6>(in, m[r]);
+        }
+        fdct_cols<6>(m);
+        for (int k = 0; k < 64; k++) b[k] = (int16_t)m[k >> 3][k & 7];
+        return;
+    }
+    const bool fast = fdct == 2;
     for (int r = 0; r < 8; r++) {
         int in[8], o[8];
         for (int k = 0; k < 8; k++) in[k] = b[8 * r + k];
@@ -150,7 +162,7 @@ __device__ inline int enc_block(const EncDev &E, int kind, const uint8_t *s1, co
         for (int x = 0; x < 8; x++) bak[8 * y + x] = t[8 * y + x] = (int16_t)((int)s1[y * stride + x] - (int)s2[y * stride + x]);     // pdsp.diff_pixels
     const bool intra = kind != 14 && S.mb_intra != 0;            // quant_psnr clears s->mb_intra first (:629)
     // ---- ff_dct_quantize_c ----
-    enc_fdct(t, S.fdct == 2);
+    enc_fdct(t, S.fdct);
     int kept_or;                                                  // (unused: these metrics never clip; n = 0, a luma block, :4389-4396)
     last = mpv_quantize(t, intra, (S.h263_aic ? 1 : S.y_dc_scale) << 3, intra ? S.q_intra_matrix : S.q_inter_matrix,
                         intra ? S.intra_quant_bias : S.inter_quant_bias, S.scantable, kept_or);
@@ -226,8 +238,8 @@ int enc_launch(int kind, int sidx, const EncDev *E, const uint8_t *cur, const ui
 
 bool state_ok(const FFMECmpEncState *s, const char *where)
 {
-    if (!s || (s->fdct != 0 && s->fdct != 2) || s->dequant < 0 || s->dequant > 3 || s->qscale < 1 || s->qscale > 31 || s->y_dc_scale < 1) {
-        set_error_msg(where, "bad encoder state (fdct 0 | 2, dequant 0..3, qscale 1..31, y_dc_scale >= 1)"); return false;
+    if (!s || (s->fdct != 0 && s->fdct != 2 && s->fdct != 6) || s->dequant < 0 || s->dequant > 3 || s->qscale < 1 || s->qscale > 31 || s->y_dc_scale < 1) {
+        set_error_msg(where, "bad encoder state (fdct 0 | 2 | 6, dequant 0..3, qscale 1..31, y_dc_scale >= 1)"); return false;
     }
     uint64_t seen = 0;
     for (int i = 0; i < 64; i++) { if (s->scantable[i] > 63) { seen = 0; break; } seen |= 1ull << s->scantable[i]; }
@@ -336,7 +348,7 @@ int ff_me_cmp_enc_init_cuda(MECmpContext *c, struct MpegEncContext *s, const FFM
                            view->block_last_index, view->q_intra_matrix, view->q_inter_matrix, view->intra_matrix, view->inter_matrix, view->scantable,
                            view->intra_ac_vlc_length, view->intra_ac_vlc_last_length, view->inter_ac_vlc_length, view->inter_ac_vlc_last_length, view->luma_dc_vlc_length };
     for (const void *p : need) if (!p) { set_error_msg("ff_me_cmp_enc_init_cuda", "a view pointer is NULL"); return -1; }
-    if (!view->idct_perm_none || !view->plain_quantiser || (view->fdct != 0 && view->fdct != 2) || view->dequant < 0 || view->dequant > 3) {
+    if (!view->idct_perm_none || !view->plain_quantiser || (view->fdct != 0 && view->fdct != 2 && view->fdct != 6) || view->dequant < 0 || view->dequant > 3) {
         set_error_msg("ff_me_cmp_enc_init_cuda", "not taken over: permuting IDCT, trellis / denoising quantiser or an unknown transform");
         return -1;
     }

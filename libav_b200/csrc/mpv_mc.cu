@@ -380,11 +380,13 @@ static int mpv_flush_run(const FFMpvPictureWork *w, const H263LfPic *lf, void *s
         if (!b.n) continue;
         int rc;
         if (b.dequant < 0)
-            rc = b.transform ? ff_xvid_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
-                             : ff_simple_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
+            rc = b.transform == 3 ? ff_faanidct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+               : b.transform      ? ff_xvid_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+                                  : ff_simple_idct_batch_cuda(b.mode, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
         else
-            rc = b.transform ? ff_mpeg_dequant_xvid_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
-                             : ff_mpeg_dequant_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
+            rc = b.transform == 3 ? ff_mpeg_dequant_faanidct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+               : b.transform      ? ff_mpeg_dequant_xvid_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream)
+                                  : ff_mpeg_dequant_idct_batch_cuda(b.dequant, b.tables, b.recs, b.blocks, b.frame, b.dst_off, b.stride, b.n, 0, b.clear, stream);
         if (rc) return -1;
     }
     if (!w->n_loop_filter) return 0;
@@ -398,9 +400,9 @@ extern "C" int ff_mpv_flush_pictures_cuda(const FFMpvPictureWork *w, void *strea
     if (!w || w->n_pictures < 0 || w->n_residual < 0 || (w->n_residual && !w->residual)) { set_error_msg(where, "bad arguments"); return -1; }
     for (int i = 0; i < w->n_residual; i++) {
         const FFMpvResidualBatch &b = w->residual[i];
-        if (b.transform < 0 || b.transform > 1 || b.dequant < -1 || b.dequant > 6 || (b.dequant < 0 && b.mode != 0 && b.mode != 1) ||
+        if (b.transform < 0 || b.transform == 2 || b.transform > 3 || b.dequant < -1 || b.dequant > 6 || (b.dequant < 0 && b.mode != 0 && b.mode != 1) ||
             (b.dequant >= 0 && (!b.tables || !b.recs)) || (b.n && (!b.blocks || !b.frame || !b.dst_off))) {
-            set_error_msg(where, "bad residual batch: transform 0 / 1, dequant -1..6, mode 0 / 1, blocks, frame and dst_off set");
+            set_error_msg(where, "bad residual batch: transform 0 / 1 / 3, dequant -1..6, mode 0 / 1, blocks, frame and dst_off set");
             return -1;
         }
     }

@@ -29,7 +29,8 @@ struct QuantDev {
 };
 struct QuantHandle {                 // what ff_mpv_quant_state_cuda returns: the device state and what the launcher needs on the host
     QuantDev *dev;
-    bool fast, has_vlc;
+    int fdct;                        // FFMpvQuantState.fdct: 0 islow, 2 ifast, 6 FAAN
+    bool has_vlc;
 };
 
 namespace {
@@ -317,8 +318,8 @@ void inv_aanscales(uint16_t *out)
 
 bool state_ok(const FFMpvQuantState *s, const char *where)
 {
-    if (!s || (s->fdct != 0 && s->fdct != 2) || s->out_format < 0 || s->out_format > 3) {
-        set_error_msg(where, "bad quantiser state (fdct 0 | 2, out_format 0..3)"); return false;
+    if (!s || (s->fdct != 0 && s->fdct != 2 && s->fdct != 6) || s->out_format < 0 || s->out_format > 3) {
+        set_error_msg(where, "bad quantiser state (fdct 0 | 2 | 6, out_format 0..3)"); return false;
     }
     uint64_t seen = 0;
     for (int i = 0; i < 64; i++) { if (s->scantable[i] > 63) { seen = 0; break; } seen |= 1ull << s->scantable[i]; }
@@ -346,7 +347,7 @@ bool make_dev(QuantDev &q, const FFMpvQuantState *st, const FFMECmpVlcTables *vl
     return true;
 }
 
-int quant_launch(const QuantDev *Q, bool fast, bool trellis, const FFMpvQuantRecord *recs, const uint8_t *s1, const uint8_t *s2, const uint32_t *off1,
+int quant_launch(const QuantDev *Q, int fdct, bool trellis, const FFMpvQuantRecord *recs, const uint8_t *s1, const uint8_t *s2, const uint32_t *off1,
                  const uint32_t *off2, ptrdiff_t stride, int16_t *blocks, size_t n, int32_t *last_index, int32_t *coded_score,
                  const FFMpvNoiseReduction *nr, bool post, cudaStream_t st, const char *where)
 {
@@ -354,8 +355,9 @@ int quant_launch(const QuantDev *Q, bool fast, bool trellis, const FFMpvQuantRec
     const uint16_t *o = nr ? nr->dct_offset : nullptr;
     int32_t *es = nr ? nr->dct_error_sum : nullptr, *ec = nr ? nr->dct_count : nullptr;
 #define QL(F, T) AVB_LAUNCH((mpv_quant_kernel<F, T>), grid, block, 0, st)(Q, recs, s1, s2, off1, off2, stride, blocks, n, last_index, coded_score, o, es, ec, post)
-    if (fast) { if (trellis) QL(2, true); else QL(2, false); }
-    else      { if (trellis) QL(0, true); else QL(0, false); }
+    if (fdct == 2)      { if (trellis) QL(2, true); else QL(2, false); }
+    else if (fdct == 6) { if (trellis) QL(6, true); else QL(6, false); }
+    else                { if (trellis) QL(0, true); else QL(0, false); }
 #undef QL
     return check_launch(where);
 }
@@ -414,7 +416,7 @@ template <bool TRELLIS> int slot_quant(struct MpegEncContext *s, int16_t *block,
     }
     if (cudaMemcpyAsync(db, hb, TOTAL, cudaMemcpyHostToDevice, st[0]) != cudaSuccess) { set_error("mpv dct_quantize slot:h2d", cudaGetLastError()); return -1; }
     const FFMpvNoiseReduction nr = { (const uint16_t *)(db + O_OFF), (int32_t *)(db + O_NR), (int32_t *)(db + O_NR + 2 * 64 * 4) };
-    if (quant_launch((const QuantDev *)(db + O_Q), v.fdct == 2, TRELLIS, (const FFMpvQuantRecord *)(db + O_REC), nullptr, nullptr, nullptr, nullptr, 0,
+    if (quant_launch((const QuantDev *)(db + O_Q), v.fdct, TRELLIS, (const FFMpvQuantRecord *)(db + O_REC), nullptr, nullptr, nullptr, nullptr, 0,
                      (int16_t *)(db + O_BLK), 1, (int32_t *)(db + O_OUT), (int32_t *)(db + O_OUT) + 1, es ? &nr : nullptr, false, st[0], where)) return -1;
     if (cudaMemcpyAsync(hb + O_BLK, db + O_BLK, TOTAL - O_BLK, cudaMemcpyDeviceToHost, st[0]) != cudaSuccess || cudaStreamSynchronize(st[0]) != cudaSuccess) {
         set_error("mpv dct_quantize slot:d2h", cudaGetLastError()); return -1;
@@ -443,7 +445,7 @@ void *ff_mpv_quant_state_cuda(const FFMpvQuantState *state, const FFMECmpVlcTabl
     avb::enter();
     QuantDev q;
     if (!make_dev(q, state, vlc, "ff_mpv_quant_state_cuda", true)) return nullptr;
-    QuantHandle *h = new QuantHandle{ nullptr, state->fdct == 2, vlc != nullptr };
+    QuantHandle *h = new QuantHandle{ nullptr, state->fdct, vlc != nullptr };
     if (cudaMalloc(&h->dev, sizeof(QuantDev)) != cudaSuccess) { set_error("ff_mpv_quant_state_cuda", cudaGetLastError()); delete h; return nullptr; }
     if (cudaMemcpy(h->dev, &q, sizeof(q), cudaMemcpyHostToDevice) != cudaSuccess) {
         set_error("ff_mpv_quant_state_cuda", cudaGetLastError()); cudaFree(h->dev); delete h; return nullptr;
@@ -472,7 +474,7 @@ int ff_mpv_dct_quantize_batch_cuda(const void *quant_state, int trellis, const F
         set_error_msg(where, "a NULL buffer (recs, blocks, last_index; off1 with s1; the three noise-reduction arrays)"); return -1;
     }
     if ((uintptr_t)blocks & 15) { set_error_msg(where, "blocks must be 16-byte aligned"); return -1; }
-    return quant_launch(h->dev, h->fast, trellis != 0, recs, s1, s2, off1, off2, stride, blocks, n, last_index, coded_score, nr, true, (cudaStream_t)stream, where);
+    return quant_launch(h->dev, h->fdct, trellis != 0, recs, s1, s2, off1, off2, stride, blocks, n, last_index, coded_score, nr, true, (cudaStream_t)stream, where);
 }
 
 int ff_mpv_quantize_init_cuda(struct MpegEncContext *s, const FFMpvQuantView *view, int trellis)
@@ -486,11 +488,11 @@ int ff_mpv_quantize_init_cuda(struct MpegEncContext *s, const FFMpvQuantView *vi
                            view->inter_ac_vlc_last_length, view->dct_error_sum, view->dct_offset, view->dct_count, view->coded_score,
                            (const void *)view->dct_quantize, (const void *)view->fast_dct_quantize };
     for (const void *p : need) if (!p) { set_error_msg(where, "a view pointer is NULL"); return -1; }
-    if (!view->idct_perm_none || (view->fdct != 0 && view->fdct != 2) || view->quantizer_noise_shaping || view->out_format < 0 || view->out_format > 3 ||
+    if (!view->idct_perm_none || (view->fdct != 0 && view->fdct != 2 && view->fdct != 6) || view->quantizer_noise_shaping || view->out_format < 0 || view->out_format > 3 ||
         view->slice_context_count != 1) {
         // (slice threading: the per-thread contexts are copies of `s` that carry the slots but not this view -- their own mb_intra,
         //  lambda2, coded_score and noise-reduction sums would be neither found nor used)
-        set_error_msg(where, "not taken over: permuting IDCT, FAAN or 10-bit transform, quantizer_noise_shaping, slice threading");
+        set_error_msg(where, "not taken over: permuting IDCT, 10-bit transform, quantizer_noise_shaping, slice threading");
         return -1;
     }
     {   // the tables the view points at: uploaded, or checked against their copy, now -- the trellis slot looks them up by address

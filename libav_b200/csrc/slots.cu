@@ -439,7 +439,7 @@ void ff_fdctdsp_init_cuda(FDCTDSPContext *c, int dct_algo, int bits_per_raw_samp
     if (high_bit_depth || bits_per_raw_sample > 8) return;               // other depths: the reference falls through to its 8-bit functions; not taken over
     if (dct_algo == AVB_FF_DCT_FASTINT) { c->fdct = slot_fdct<2>; c->fdct248 = slot_fdct<3>; }
     else if (dct_algo == AVB_FF_DCT_AUTO || dct_algo == AVB_FF_DCT_INT) { c->fdct = slot_fdct<0>; c->fdct248 = slot_fdct<1>; }
-    // FF_DCT_FAAN (float) is not taken over
+    else if (dct_algo == AVB_FF_DCT_FAAN) { c->fdct = slot_fdct<6>; c->fdct248 = slot_fdct<7>; }
 }
 
 void ff_me_cmp_init_cuda(MECmpContext *c)
