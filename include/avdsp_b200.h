@@ -36,7 +36,9 @@ int         avb200_init(int device);              /* cudaSetDevice + context war
 const char *avb200_last_error(void);              /* "" when no error is pending */
 void        avb200_clear_error(void);
 void        avb200_set_log_callback(void (*cb)(int av_log_level, const char *msg)); /* av_log-style sink */
-void        avb200_set_tuning(const char *key, int value);   /* kernel-variant knobs for profiling; see DESIGN.md */
+void        avb200_set_tuning(const char *key, int value);   /* test knobs that force a fallback kernel the library picks for other
+                                                               inputs: sws_general_variant, mc_variant, residual_variant, idct_tma
+                                                               (0 = the default); unknown keys are ignored */
 void       *avb200_malloc(size_t bytes);          /* device memory */
 void        avb200_free(void *dptr);
 void       *avb200_host_alloc(size_t bytes);      /* pinned host memory */

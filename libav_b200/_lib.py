@@ -163,7 +163,7 @@ def init(device=0):
     if device not in _initialised:
         check(lib.avb200_init(device), "avb200_init(%d)" % device)
         _initialised[device] = True
-        for kv in filter(None, os.environ.get("AVB200_TUNE", "").split(",")):     # profiling knobs, e.g. sws_fused_variant=3
+        for kv in filter(None, os.environ.get("AVB200_TUNE", "").split(",")):     # test knobs, e.g. mc_variant=2
             k, v = kv.split("=")
             lib.avb200_set_tuning(k.encode(), int(v))
     return True

@@ -27,7 +27,7 @@ int  check_launch(const char *where);   // cudaGetLastError() -> sticky error, r
 
 void enter();                   // make the device avb200_init() chose current in the calling thread (first statement of every public entry point)
 int sm_count();                 // multiprocessor count of the current device (cached)
-int tuning(const char *key);    // experiment knob set through avb200_set_tuning(); 0 when unset
+int tuning(const char *key);    // test knob set through avb200_set_tuning(); 0 when unset
 
 // ---- device helpers ------------------------------------------------------------------------
 #ifdef AVB_HOSTSIM

@@ -14,8 +14,7 @@ namespace avb {
 
 namespace {
 
-template <int MINB>
-__global__ void __launch_bounds__(128, MINB)
+__global__ void __launch_bounds__(128, 6)
 h264_mc_kernel_v2(const FFH264MCRecord *__restrict__ recs, size_t n, const FFH264RefPlanes *__restrict__ refs,
                   uint8_t *__restrict__ dy, uint8_t *__restrict__ dcb, uint8_t *__restrict__ dcr, int ls, int uvls, int pw, int ph, int pass)
 {
@@ -123,13 +122,7 @@ int launch_h264_mc_v2(const FFH264MCRecord *recs, size_t n, const FFH264RefPlane
     // compiled for 6 resident CTAs per SM (80 registers, ~40 words of spill that stay in L1): the kernel waits on its patch loads, so warps
     // in flight count for more than registers, up to the point where spills cost more -- bench.py --workload h264 on an H100 80GB HBM3
     // (700 W): 4 CTAs (128 registers) 3.85 ms per step, 6 CTAs 3.76 ms, 8 CTAs (64 registers, ~110 words of spill) 4.09 ms.
-    // mc_min_blocks = 4 / 8: profiling
-    const int minb = tuning("mc_min_blocks");
-    for (int pass = 0; pass < 2; pass++) {
-        if (minb == 4)      h264_mc_kernel_v2<4><<<grid, 128, 0, st>>>(recs, n, refs, dy, dcb, dcr, ls, uvls, pw, ph, pass);
-        else if (minb == 8) h264_mc_kernel_v2<8><<<grid, 128, 0, st>>>(recs, n, refs, dy, dcb, dcr, ls, uvls, pw, ph, pass);
-        else                h264_mc_kernel_v2<6><<<grid, 128, 0, st>>>(recs, n, refs, dy, dcb, dcr, ls, uvls, pw, ph, pass);
-    }
+    for (int pass = 0; pass < 2; pass++) h264_mc_kernel_v2<<<grid, 128, 0, st>>>(recs, n, refs, dy, dcb, dcr, ls, uvls, pw, ph, pass);
     return check_launch("h264_mc_batch") ? -1 : 0;
 }
 

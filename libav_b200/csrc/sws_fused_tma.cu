@@ -5,18 +5,18 @@
 // evaluated arithmetically.  What changes is how the bytes travel and how many instructions a pixel costs:
 //   * a warp owns a 256 x 8 pixel tile (four row pairs).  Its luma rows (8 x 256 B) and the eight chroma lines of each plane that the
 //     tile's vertical windows touch (8 x 128 B each) arrive by three cp.async.bulk.tensor (TMA, 3-D maps x / line / frame, zero fill
-//     outside the plane) into one of the warp's own 2 or 3 stages and are awaited on that stage's mbarrier: no CTA-wide barrier exists
-//     after start-up, the next two tiles (or the next one) are always in flight.  Warps are persistent and stride over the tiles of all
-//     frames of the batch.
+//     outside the plane) into one of the warp's own three stages and are awaited on that stage's mbarrier: no CTA-wide barrier exists
+//     after start-up, the next two tiles are always in flight.  Warps are persistent and stride over the tiles of all frames of the
+//     batch.
 //   * a thread owns 16 pixels x 4 rows (row pairs `half` and `half + 2` of the tile).  The seven chroma lines they need are
 //     byte-transposed once (window 0-3), the windows of the next rows are one PRMT away (drop the oldest line, append the next); the
 //     4-tap FIR is two IDP.2A on int16 taps.
 //   * the rows leave through shared memory: four 768-byte rows per cp.async.bulk.tensor store (whole 128-byte lines per request).
 //   * the per-(U, V) additive terms  cy * ((V * crv) >> 16) + kr,  cy * ((V * cgv) >> 16),  cy * ((U * cbu) >> 16) + kb,
 //     cy * ((U * cgu) >> 16) + kg  come from two 256-entry tables in shared memory, built by the CTA from the context's constants
-//     with exactly these formulas, 16 copies of each 8-byte entry so that every lane of a half-warp reads its own bank pair
-//     (conflict-free whatever the picture holds): 2 LDS.64 + 1 IADD instead of 12 integer instructions per chroma sample and row.
-//     With three stages per warp the shared memory holds 8 copies (at most a 2-way bank conflict).
+//     with exactly these formulas, 8 copies of each 8-byte entry so that every pair of lanes of a half-warp reads its own bank pair
+//     (at most a 2-way bank conflict whatever the picture holds; 16 conflict-free copies leave no room for the third stage):
+//     2 LDS.64 + 1 IADD instead of 12 integer instructions per chroma sample and row.
 //   * luma loads and output stores carry an L2 evict-first policy: both are touched once, while the chroma lines are read again by the
 //     next tile row.
 //   * the launch is a programmatic dependent of the one before it on the stream: its CTAs build their tables while that launch drains,
@@ -31,13 +31,17 @@ namespace avb {
 namespace {
 
 constexpr int FT_STAGE = 4096;                  // Y 8 rows x 256 B | U 8 lines x 128 B | V 8 lines x 128 B
+constexpr int FT_STAGES = 3;                    // tile stages per warp
 constexpr int FT_OUT = 4 * 768;                 // output staging: four 768-byte rows (half a tile) per bulk tensor store
-constexpr int FT_MAX_WARPS = 14;                // the largest CTA (sws_tma_warps)
+constexpr int FT_LUTC = 8;                      // lane copies of each term table entry
+constexpr int FT_LUT_BYTES = 2 * 256 * FT_LUTC * 8;     // table by V {tr, tgv}, table by U {tb, tgu}: 256 entries x FT_LUTC copies x 8 B
+constexpr int FT_MAX_WARPS = 12;                // the largest CTA
 constexpr int FT_SMEM_MAX = 227 * 1024;         // shared memory a CTA may opt in to on sm_90
-// table by V {tr, tgv}, table by U {tb, tgu}: 256 entries x LUTC lane copies x 8 B
-__host__ __device__ constexpr int ft_lut_bytes(bool lut, int lutc) { return lut ? 2 * 256 * lutc * 8 : 0; }
-__host__ __device__ constexpr int ft_smem_bytes(bool lut, int lutc, int stages, int warps)
-{ return ft_lut_bytes(lut, lutc) + warps * (stages * FT_STAGE + FT_OUT + 8 * stages); }
+// The launch bound keeps the register budget of a 14-warp CTA, which the kernel's schedule was measured under (profiles/README.md):
+// a 12-warp bound gives the same 127 registers but another instruction schedule.
+constexpr int FT_BOUND_THREADS = 14 * 32;
+constexpr int ft_smem_bytes(int warps) { return FT_LUT_BYTES + warps * (FT_STAGES * FT_STAGE + FT_OUT + 8 * FT_STAGES); }
+static_assert(ft_smem_bytes(FT_MAX_WARPS) <= FT_SMEM_MAX, "the largest CTA's stages, slabs and tables must fit in shared memory");
 
 struct FusedTmaArgs {
     uint8_t *dst; int dstStride; size_t dstFrame;
@@ -46,7 +50,6 @@ struct FusedTmaArgs {
     int tilesX, nTy;                  // tiles per tile row, tile rows of the launch
     int nitems;                       // nframes * nTy * tilesX
     int stepX, stepTy, stepF;         // the (tx, ty, frame) decomposition of the warp stride gridDim.x * warps
-    int hint;                         // L2 evict-first on the luma loads and the output stores
 };
 
 __device__ __forceinline__ int dp2a_lo(uint32_t k, uint32_t b, int c)
@@ -66,11 +69,10 @@ __device__ __forceinline__ void slide4(const uint32_t *w, uint32_t next, uint32_
 { out[0] = slide<0>(w[0], next); out[1] = slide<1>(w[1], next); out[2] = slide<2>(w[2], next); out[3] = slide<3>(w[3], next); }
 
 // one output row of 16 pixels: TU / TV = the row's four chroma lines of each of the 8 chroma columns, yy = 16 luma bytes
-template <bool BGR, bool LUT, int LUTC>
+template <bool BGR>
 __device__ __forceinline__ void row16(const uint32_t (&TU)[8], const uint32_t (&TV)[8], uint32_t k01, uint32_t k23, uint4 yy,
-                                      const RgbConstants &k, unsigned lutU_s, unsigned lutV_s, uint32_t (&o)[12])
+                                      int cy, unsigned lutU_s, unsigned lutV_s, uint32_t (&o)[12])
 {
-    const int cy = k.cy;
 #pragma unroll
     for (int q = 0; q < 4; q++) {                            // 4 pixels = 2 chroma columns per step
         const uint32_t yw = q == 0 ? yy.x : q == 1 ? yy.y : q == 2 ? yy.z : yy.w;
@@ -82,15 +84,8 @@ __device__ __forceinline__ void row16(const uint32_t (&TU)[8], const uint32_t (&
             const int su = dp2a_hi(k23, TU[c], dp2a_lo(k01, TU[c], 2048));
             const int sv = dp2a_hi(k23, TV[c], dp2a_lo(k01, TV[c], 2048));
             const int U = sat255(su >> 12), V = sat255(sv >> 12);        // per-value clip == the reference's flagged clip (host-checked range)
-            int tr, tg, tb;
-            if (LUT) {
-                const uint2 lv = lds64_ro(lutV_s + V * (LUTC * 8)), lu = lds64_ro(lutU_s + U * (LUTC * 8));
-                tr = (int)lv.x; tb = (int)lu.x; tg = (int)(lu.y + lv.y);
-            } else {
-                tr = cy * ((V * k.crv) >> 16) + k.kr;
-                tg = cy * (((U * k.cgu) >> 16) + ((V * k.cgv) >> 16)) + k.kg;
-                tb = cy * ((U * k.cbu) >> 16) + k.kb;
-            }
+            const uint2 lv = lds64_ro(lutV_s + V * (FT_LUTC * 8)), lu = lds64_ro(lutU_s + U * (FT_LUTC * 8));
+            const int tr = (int)lv.x, tb = (int)lu.x, tg = (int)(lu.y + lv.y);
             const int Ya = byte_of(yw, 2 * e), Yb = byte_of(yw, 2 * e + 1);
             r[2 * e] = cy * Ya + (BGR ? tb : tr); g[2 * e] = cy * Ya + tg; b[2 * e] = cy * Ya + (BGR ? tr : tb);
             r[2 * e + 1] = cy * Yb + (BGR ? tb : tr); g[2 * e + 1] = cy * Yb + tg; b[2 * e + 1] = cy * Yb + (BGR ? tr : tb);
@@ -101,46 +96,41 @@ __device__ __forceinline__ void row16(const uint32_t (&TU)[8], const uint32_t (&
     }
 }
 
-// LUTC lane copies per table entry (16 or 8), STAGES tile stages per warp (2 or 3).
-// MOVE: a ceiling probe, not a scaler -- the same grid, tile order, loads, waits and stores, but the "pixels" it stores are the staged
-// luma bytes (a wrong picture on purpose); reached only through the sws_tma_probe knob.
-template <bool BGR, bool LUT, int LUTC, int STAGES, bool MOVE>
-__global__ void __launch_bounds__(FT_MAX_WARPS * 32, 1)
+template <bool BGR>
+__global__ void __launch_bounds__(FT_BOUND_THREADS, 1)
 sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const SwsPairTapsT *__restrict__ taps,
                            const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmV,
                            const __grid_constant__ CUtensorMap tmD)
 {
     extern __shared__ __align__(1024) uint8_t ft_smem[];
-    constexpr int LUT_BYTES = ft_lut_bytes(LUT, LUTC);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     const unsigned smem_s = (unsigned)__cvta_generic_to_shared(ft_smem);
-    const unsigned stage_s = smem_s + LUT_BYTES + warp * STAGES * FT_STAGE;
-    const unsigned out_s = smem_s + LUT_BYTES + nwarps * STAGES * FT_STAGE + warp * FT_OUT;
-    const unsigned mbar_s = smem_s + LUT_BYTES + nwarps * (STAGES * FT_STAGE + FT_OUT) + warp * 8 * STAGES;
+    const unsigned stage_s = smem_s + FT_LUT_BYTES + warp * FT_STAGES * FT_STAGE;
+    const unsigned out_s = smem_s + FT_LUT_BYTES + nwarps * FT_STAGES * FT_STAGE + warp * FT_OUT;
+    const unsigned mbar_s = smem_s + FT_LUT_BYTES + nwarps * (FT_STAGES * FT_STAGE + FT_OUT) + warp * 8 * FT_STAGES;
 
-    if (LUT && !MOVE) {                 // the two term tables, every entry LUTC times (one copy per lane of a half-warp, or per pair of lanes)
-        uint2 *lut = reinterpret_cast<uint2 *>(ft_smem);
-        for (int e = threadIdx.x; e < 2 * 256 * LUTC; e += blockDim.x) {
-            const int i = (e / LUTC) & 255;
-            uint2 val;
-            if (e < 256 * LUTC) { val.x = (uint32_t)(k.cy * ((i * k.crv) >> 16) + k.kr); val.y = (uint32_t)(k.cy * ((i * k.cgv) >> 16)); }
-            else                { val.x = (uint32_t)(k.cy * ((i * k.cbu) >> 16) + k.kb); val.y = (uint32_t)(k.cy * ((i * k.cgu) >> 16) + k.kg); }
-            lut[e] = val;
-        }
+    // the two term tables, every entry FT_LUTC times (one copy per pair of lanes of a half-warp)
+    uint2 *lut = reinterpret_cast<uint2 *>(ft_smem);
+    for (int e = threadIdx.x; e < 2 * 256 * FT_LUTC; e += blockDim.x) {
+        const int i = (e / FT_LUTC) & 255;
+        uint2 val;
+        if (e < 256 * FT_LUTC) { val.x = (uint32_t)(k.cy * ((i * k.crv) >> 16) + k.kr); val.y = (uint32_t)(k.cy * ((i * k.cgv) >> 16)); }
+        else                   { val.x = (uint32_t)(k.cy * ((i * k.cbu) >> 16) + k.kb); val.y = (uint32_t)(k.cy * ((i * k.cgu) >> 16) + k.kg); }
+        lut[e] = val;
     }
     if (lane == 0) {
 #pragma unroll
-        for (int s = 0; s < STAGES; s++) mbar_init(mbar_s + 8 * s, 1);
+        for (int s = 0; s < FT_STAGES; s++) mbar_init(mbar_s + 8 * s, 1);
         mbar_init_fence();
     }
     __syncthreads();
     // Launched as a programmatic dependent of the previous launch on the stream, the CTA gets here (tables built, barriers set up)
-    // while that launch drains; nothing in global memory is touched before it has completed.  Both are no-ops otherwise.
+    // while that launch drains; nothing in global memory is touched before it has completed.
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
     const int cg = lane & 15, half = lane >> 4;
-    const unsigned lutV_s = smem_s + (cg % LUTC) * 8, lutU_s = smem_s + 256 * LUTC * 8 + (cg % LUTC) * 8;
+    const unsigned lutV_s = smem_s + (cg % FT_LUTC) * 8, lutU_s = smem_s + 256 * FT_LUTC * 8 + (cg % FT_LUTC) * 8;
 
     int item = blockIdx.x * nwarps + warp;
     if (item >= a.nitems) return;
@@ -158,21 +148,20 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
             const unsigned mb = mbar_s + 8 * st, dst = stage_s + st * FT_STAGE;
             fence_proxy_async();                              // the stage was last read by ordinary shared loads
             mbar_expect_tx(mb, FT_STAGE);
-            if (a.hint) tma_load_3d_hint(dst, &tmY, tx * 256, 2 * (a.rp0 + 4 * ty), f, mb, evict_first);
-            else        tma_load_3d(dst, &tmY, tx * 256, 2 * (a.rp0 + 4 * ty), f, mb);
+            tma_load_3d_hint(dst, &tmY, tx * 256, 2 * (a.rp0 + 4 * ty), f, mb, evict_first);
             tma_load_3d(dst + 2048, &tmU, tx * 128, base, f, mb);
             tma_load_3d(dst + 3072, &tmV, tx * 128, base, f, mb);
         }
     };
-    // The tile being computed (c) and the tile issued next (n, STAGES - 1 strides ahead) are tracked by coordinates; the table words of
-    // n are fetched a whole tile before its loads are issued, those of the tiles in flight are kept in q (oldest first).
+    // The tile being computed (c) and the tile issued next (n, FT_STAGES - 1 strides ahead) are tracked by coordinates; the table words
+    // of n are fetched a whole tile before its loads are issued, those of the tiles in flight are kept in q (oldest first).
     int ctx = item % a.tilesX, cty, cf;
     { const int t2 = item / a.tilesX; cty = t2 % a.nTy; cf = t2 / a.nTy; }
     int ntx = ctx, nty = cty, nf = cf;
     long long nitem = item;
-    int2 q[STAGES - 1];
+    int2 q[FT_STAGES - 1];
 #pragma unroll
-    for (int s = 0; s < STAGES - 1; s++) {
+    for (int s = 0; s < FT_STAGES - 1; s++) {
         q[s] = nitem < a.nitems ? tile_words(nty) : make_int2(0, 0);
         if (nitem < a.nitems) issue(ntx, nty, nf, q[s].x, s);
         advance(ntx, nty, nf); nitem += wstride;
@@ -182,11 +171,11 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
     unsigned st = 0, phase = 0;
     for (; item < a.nitems; item += wstride) {
         const int2 cw = q[0];
-        // the stage computed last (st - 1) is free again: the tile STAGES - 1 strides ahead starts travelling before this one is touched
-        if (nitem < a.nitems) issue(ntx, nty, nf, nw.x, st == 0 ? STAGES - 1 : st - 1);
+        // the stage computed last (st - 1) is free again: the tile FT_STAGES - 1 strides ahead starts travelling before this one is touched
+        if (nitem < a.nitems) issue(ntx, nty, nf, nw.x, st == 0 ? FT_STAGES - 1 : st - 1);
 #pragma unroll
-        for (int s = 0; s < STAGES - 2; s++) q[s] = q[s + 1];
-        q[STAGES - 2] = nw;
+        for (int s = 0; s < FT_STAGES - 2; s++) q[s] = q[s + 1];
+        q[FT_STAGES - 2] = nw;
         advance(ntx, nty, nf); nitem += wstride;
         nw = nitem < a.nitems ? tile_words(nty) : make_int2(0, 0);
 
@@ -206,25 +195,12 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) {
-                if (a.hint) tma_store_3d_hint(&tmD, ctx * 192, 2 * rpT + 4 * g, cf, out_s, evict_first);
-                else        tma_store_3d(&tmD, ctx * 192, 2 * rpT + 4 * g, cf, out_s);
+                tma_store_3d_hint(&tmD, ctx * 192, 2 * rpT + 4 * g, cf, out_s, evict_first);
                 bulk_commit();
             }
         };
 
-        if (MOVE) {
-            // probe: each half-tile slab (3072 B) is filled with the half-tile's luma rows (1024 B) three times over
-#pragma unroll
-            for (int g = 0; g < 2; g++) {
-                slab_free();
-#pragma unroll
-                for (int j = 0; j < 6; j++) {
-                    const int i = lane + 32 * j;
-                    sts128(out_s + 16 * i, lds128(sY + 1024 * g + 16 * (i & 63)));
-                }
-                flush(g);
-            }
-        } else if (cw.y) {
+        if (cw.y) {
             // interior tile: pair q of the tile filters chroma lines q .. q + 3 (first row) and q + 1 .. q + 4 (second row) of the stage.
             // This thread's pairs are `half` and `half + 2`: seven lines, four windows one line apart
             uint4 yy[4];
@@ -239,16 +215,16 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
             transpose4(ul[0].x, ul[1].x, ul[2].x, ul[3].x, WU); transpose4(ul[0].y, ul[1].y, ul[2].y, ul[3].y, WU + 4);
             transpose4(vl[0].x, vl[1].x, vl[2].x, vl[3].x, WV); transpose4(vl[0].y, vl[1].y, vl[2].y, vl[3].y, WV + 4);
             slab_free();
-            row16<BGR, LUT, LUTC>(WU, WV, tA.x, tA.y, yy[0], k, lutU_s, lutV_s, o); stage_row(2 * half, o);
+            row16<BGR>(WU, WV, tA.x, tA.y, yy[0], k.cy, lutU_s, lutV_s, o); stage_row(2 * half, o);
             slide4(WU, ul[4].x, XU); slide4(WU + 4, ul[4].y, XU + 4); slide4(WV, vl[4].x, XV); slide4(WV + 4, vl[4].y, XV + 4);
-            row16<BGR, LUT, LUTC>(XU, XV, tA.z, tA.w, yy[1], k, lutU_s, lutV_s, o); stage_row(2 * half + 1, o);
+            row16<BGR>(XU, XV, tA.z, tA.w, yy[1], k.cy, lutU_s, lutV_s, o); stage_row(2 * half + 1, o);
             flush(0);
             slide4(XU, ul[5].x, WU); slide4(XU + 4, ul[5].y, WU + 4); slide4(XV, vl[5].x, WV); slide4(XV + 4, vl[5].y, WV + 4);
-            row16<BGR, LUT, LUTC>(WU, WV, tB.x, tB.y, yy[2], k, lutU_s, lutV_s, o);
+            row16<BGR>(WU, WV, tB.x, tB.y, yy[2], k.cy, lutU_s, lutV_s, o);
             slab_free();
             stage_row(2 * half, o);
             slide4(WU, ul[6].x, XU); slide4(WU + 4, ul[6].y, XU + 4); slide4(WV, vl[6].x, XV); slide4(WV + 4, vl[6].y, XV + 4);
-            row16<BGR, LUT, LUTC>(XU, XV, tB.z, tB.w, yy[3], k, lutU_s, lutV_s, o); stage_row(2 * half + 1, o);
+            row16<BGR>(XU, XV, tB.z, tB.w, yy[3], k.cy, lutU_s, lutV_s, o); stage_row(2 * half + 1, o);
             flush(1);
         } else {
             // plane edges and ragged tiles: every row fetches its own four (clamped) lines
@@ -269,7 +245,7 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
                 uint32_t TU[8], TV[8], o[12];
                 transpose4(ul[0].x, ul[1].x, ul[2].x, ul[3].x, TU); transpose4(ul[0].y, ul[1].y, ul[2].y, ul[3].y, TU + 4);
                 transpose4(vl[0].x, vl[1].x, vl[2].x, vl[3].x, TV); transpose4(vl[0].y, vl[1].y, vl[2].y, vl[3].y, TV + 4);
-                row16<BGR, LUT, LUTC>(TU, TV, kk.x, kk.y, yy, k, lutU_s, lutV_s, o);
+                row16<BGR>(TU, TV, kk.x, kk.y, yy, k.cy, lutU_s, lutV_s, o);
                 if (!(r & 1)) slab_free();
                 stage_row(trow & 3, o);
                 if (r & 1) flush(r >> 1);
@@ -277,74 +253,12 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
             __syncwarp();
         }
         advance(ctx, cty, cf);
-        if (++st == STAGES) { st = 0; phase ^= 1u; }
+        if (++st == FT_STAGES) { st = 0; phase ^= 1u; }
     }
     if (lane == 0) bulk_wait<0>();
 }
 
-// Ceiling probe, not a scaler: streams the batch's Y, U and V bytes in and as many output bytes as the real call out, 16 bytes per
-// access, both linear -- a wrong picture on purpose; reached only through the sws_tma_probe knob.  Input chunk i is written to output
-// chunks i and i + half; a thread keeps four loads in flight.
-__global__ void __launch_bounds__(512)
-sws_flat_stream_probe_kernel(const uint4 *__restrict__ y, const uint4 *__restrict__ u, const uint4 *__restrict__ v, uint4 *__restrict__ dst,
-                             long long nY, long long nU, long long nV, long long nOut)
-{
-    const long long nIn = nY + nU + nV, half = (nOut + 1) / 2, n = nIn > half ? nIn : half;
-    const long long stride = (long long)gridDim.x * blockDim.x;
-    for (long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x; i0 < n; i0 += 4 * stride) {
-        uint4 w[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const long long i = i0 + j * stride;
-            w[j] = i < nY ? __ldg(y + i) : i < nY + nU ? __ldg(u + (i - nY)) : i < nIn ? __ldg(v + (i - nY - nU)) : make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const long long i = i0 + j * stride;
-            if (i < nOut) dst[i] = w[j];
-            if (i + half < nOut) dst[i + half] = w[j];
-        }
-    }
-}
-
 }  // namespace
-
-// the grid, the (tx, ty, frame) steps of the warp stride and the launch of one kernel shape; `max_ctas` = the CTAs the work can use
-template <bool BGR, bool LUT, int LUTC, int STAGES, bool MOVE>
-static int launch_variant(const RgbConstants &k, FusedTmaArgs fa, const SwsPairTapsT *taps, const CUtensorMap &tmY, const CUtensorMap &tmU,
-                          const CUtensorMap &tmV, const CUtensorMap &tmD, int warps, long long max_ctas, bool pdl, cudaStream_t st)
-{
-    auto kern = sws_fused_rgb24_tma_kernel<BGR, LUT, LUTC, STAGES, MOVE>;
-    const int smem = ft_smem_bytes(LUT, LUTC, STAGES, warps);
-    static int attr_smem = 0;                       // the largest dynamic shared memory this shape has been allowed so far
-    static int ctas_per_sm[FT_MAX_WARPS + 1] = {};
-    if (smem > attr_smem) {
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-            set_error("sws_scale:fused tma", cudaGetLastError()); return -1;
-        }
-        attr_smem = smem;
-    }
-    if (!ctas_per_sm[warps]) {
-        int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, warps * 32, smem) != cudaSuccess || n <= 0) {
-            set_error_msg("sws_scale:fused tma", "kernel shape does not fit an SM"); cudaGetLastError(); return -1;
-        }
-        ctas_per_sm[warps] = n;
-    }
-    long long grid = (long long)sm_count() * ctas_per_sm[warps];
-    if (grid > max_ctas) grid = max_ctas;
-    const long long wstride = grid * warps;
-    fa.stepX = (int)(wstride % fa.tilesX);
-    { const long long t2 = wstride / fa.tilesX; fa.stepTy = (int)(t2 % fa.nTy); fa.stepF = (int)(t2 / fa.nTy); }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(warps * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    if (cudaLaunchKernelEx(&cfg, kern, k, fa, taps, tmY, tmU, tmV, tmD) != cudaSuccess) { set_error("sws_scale:fused tma", cudaGetLastError()); return -1; }
-    return check_launch("sws_scale:fused tma");
-}
 
 int sws_fused_tma_launch(const RgbConstants &k, int bgr, int dstW, int dstH, int chrSrcW, int chrSrcH, const FusedArgs &a,
                          const SwsPairTapsT *taps, int nframes, cudaStream_t st)
@@ -358,21 +272,6 @@ int sws_fused_tma_launch(const RgbConstants &k, int bgr, int dstW, int dstH, int
     if ((a.yStride | a.uStride | a.vStride | a.dstStride) & 15) return 1;
     if (nframes > 1 && ((a.yFrame | a.uFrame | a.vFrame | a.dstFrame) & 15)) return 1;
     if (a.yStride <= 0 || a.uStride <= 0 || a.vStride <= 0) return 1;
-    // Tuning knobs (profiling; 0 = the default):
-    //   sws_tma_warps   4 / 12 / 14 warps per CTA (default: 12, or 4 for batches of fewer than two rounds of tiles)
-    //   sws_tma_stages  2 / 3 tile stages per warp (default 3 where the shared memory holds them, with 8 lane copies of the tables)
-    //   sws_tma_hint    1 = no L2 hints, 2 = evict-first luma loads and output stores (default)
-    //   sws_tma_pdl     1 = plain launch, 2 = programmatic dependent launch (default)
-    //   sws_tma_lut     2 = arithmetic terms instead of the shared-memory tables (2 stages)
-    //   sws_tma_probe   1 = move-only, 2 = flat stream: ceiling probes that write wrong pictures on purpose
-    // sws_tma_stages=2, sws_tma_hint=1, sws_tma_pdl=1 is the kernel as it was before three stages, L2 hints and dependent launches.
-    if (tuning("sws_tma_probe") == 2) {
-        auto bytes = [&](size_t frame, int stride, int h) { return (long long)((nframes > 1 ? frame * nframes : (size_t)stride * h) / 16); };
-        const long long nY = bytes(a.yFrame, a.yStride, dstH), nU = bytes(a.uFrame, a.uStride, chrSrcH), nV = bytes(a.vFrame, a.vStride, chrSrcH);
-        const long long nOut = bytes(a.dstFrame, a.dstStride, dstH);
-        sws_flat_stream_probe_kernel<<<sm_count() * 4, 512, 0, st>>>((const uint4 *)a.y, (const uint4 *)a.u, (const uint4 *)a.v, (uint4 *)a.dst, nY, nU, nV, nOut);
-        return check_launch("sws_scale:flat stream probe");
-    }
     CUtensorMap tmY, tmU, tmV, tmD;
     {
         // the destination as 32-bit words: a 256-pixel row of a tile is 768 bytes = 192 words (a box side is at most 256 elements)
@@ -399,23 +298,42 @@ int sws_fused_tma_launch(const RgbConstants &k, int bgr, int dstW, int dstH, int
     if (nitems > 0x7fffffff / 2) return 1;
     fa.nitems = (int)nitems;
 
-    const bool lut = tuning("sws_tma_lut") != 2;
-    int warps = tuning("sws_tma_warps");
-    if (warps != 4 && warps != 12 && warps != 14) warps = nitems >= 12 * 2 * sm_count() ? 12 : 4;
-    if (!lut && warps == 14) warps = 12;
-    const int stages = lut && tuning("sws_tma_stages") != 2 && ft_smem_bytes(true, 8, 3, warps) <= FT_SMEM_MAX ? 3 : 2;
-    fa.hint = tuning("sws_tma_hint") != 1;
-    const bool pdl = tuning("sws_tma_pdl") != 1;
+    // 12 warps per CTA (one CTA per SM); batches of fewer than two tiles per warp of that grid take 4-warp CTAs, which spread them over
+    // more SMs
+    const int warps = nitems >= 12 * 2 * sm_count() ? 12 : 4;
+    const int smem = ft_smem_bytes(warps);
+    const int b = bgr ? 1 : 0;
+    auto kern = b ? sws_fused_rgb24_tma_kernel<true> : sws_fused_rgb24_tma_kernel<false>;
+    static int attr_smem[2] = {};                   // the largest dynamic shared memory each kernel has been allowed so far
+    static int ctas_per_sm[2][FT_MAX_WARPS + 1] = {};
+    if (smem > attr_smem[b]) {
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+            set_error("sws_scale:fused tma", cudaGetLastError()); return -1;
+        }
+        attr_smem[b] = smem;
+    }
+    if (!ctas_per_sm[b][warps]) {
+        int n = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, warps * 32, smem) != cudaSuccess || n <= 0) {
+            set_error_msg("sws_scale:fused tma", "kernel shape does not fit an SM"); cudaGetLastError(); return -1;
+        }
+        ctas_per_sm[b][warps] = n;
+    }
+    // the grid (no more CTAs than the work can use) and the (tx, ty, frame) steps of the warp stride
     const long long max_ctas = (nitems + warps - 1) / warps;
-    const bool move = tuning("sws_tma_probe") == 1;
-#define AVB_FT_GO(BGR, L, C, S) launch_variant<BGR, L, C, S, false>(k, fa, taps, tmY, tmU, tmV, tmD, warps, max_ctas, pdl, st)
-#define AVB_FT_MOVE(C, S) launch_variant<false, true, C, S, true>(k, fa, taps, tmY, tmU, tmV, tmD, warps, max_ctas, pdl, st)
-    if (move) return stages == 3 ? AVB_FT_MOVE(8, 3) : AVB_FT_MOVE(16, 2);
-    if (!lut) return bgr ? AVB_FT_GO(true, false, 16, 2) : AVB_FT_GO(false, false, 16, 2);
-    if (stages == 3) return bgr ? AVB_FT_GO(true, true, 8, 3) : AVB_FT_GO(false, true, 8, 3);
-    return bgr ? AVB_FT_GO(true, true, 16, 2) : AVB_FT_GO(false, true, 16, 2);
-#undef AVB_FT_GO
-#undef AVB_FT_MOVE
+    long long grid = (long long)sm_count() * ctas_per_sm[b][warps];
+    if (grid > max_ctas) grid = max_ctas;
+    const long long wstride = grid * warps;
+    fa.stepX = (int)(wstride % fa.tilesX);
+    { const long long t2 = wstride / fa.tilesX; fa.stepTy = (int)(t2 % fa.nTy); fa.stepF = (int)(t2 / fa.nTy); }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(warps * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    if (cudaLaunchKernelEx(&cfg, kern, k, fa, taps, tmY, tmU, tmV, tmD) != cudaSuccess) { set_error("sws_scale:fused tma", cudaGetLastError()); return -1; }
+    return check_launch("sws_scale:fused tma");
 }
 
 }  // namespace avb

@@ -1850,7 +1850,7 @@ static int launch_fused_fast(SwsCudaContext *c, const FusedArgs &a, int nframes,
 {
     const SwsDev &p = c->dev;
 #ifndef AVB_HOSTSIM
-    if (c->tma_ok && tuning("sws_fused_variant") != 3) {
+    if (c->tma_ok) {
         const int r = sws_fused_tma_launch(p.k, p.bgr, p.dstW, p.dstH, p.chrSrcW, p.chrSrcH, a, (const SwsPairTapsT *)c->d_pair_taps_t, nframes, st);
         if (r <= 0) return r;
     }
@@ -1876,7 +1876,7 @@ static int run_fused(SwsCudaContext *c, const uint8_t *const src[3], const int s
     const bool a16 = aligned && !((uintptr_t)a.y & 15) && !(a.yStride & 15) && !((uintptr_t)a.dst & 15) && !(a.dstStride & 15) &&
                      !(a.yFrame & 15) && !(a.dstFrame & 15) && !((uintptr_t)a.u & 7) && !((uintptr_t)a.v & 7) && !(a.uStride & 7) &&
                      !(a.vStride & 7) && !(a.uFrame & 7) && !(a.vFrame & 7) && !((uintptr_t)p.vChrF & 15);
-    if (c->fast_ok && a16 && tuning("sws_fused_variant") != 1) {
+    if (c->fast_ok && a16) {
         a.rp0 = 0; a.rp1 = p.dstH / 2;
         return launch_fused_fast(c, a, nframes, st);
     }
@@ -2454,12 +2454,12 @@ static int scale_host(SwsCudaContext *c, const uint8_t *const srcSlice[], const 
     if (grow(c->d_src, c->src_bytes, sOff[3], s, "sws_scale_cuda") || grow(c->d_dst, c->dst_bytes, dOff[3], s, "sws_scale_cuda")) return 0;
     const uint8_t *ds[3] = { c->d_src, c->S->fam == FAM_PAL8 ? c->d_pal : c->d_src + sOff[1], c->d_src + sOff[2] };     // (pal8: plane 1 is the palette)
     uint8_t *dd[3] = { c->d_dst, c->d_dst + dOff[1], c->d_dst + dOff[2] };
-    // Same-size rgb (the dp4a fused kernel): the frame goes through in bands of rows on three streams, so the upload of band
-    // k + 1, the kernel of band k and the download of band k - 1 overlap -- the call is PCIe bound and PCIe is full duplex.
+    // Same-size rgb (the dp4a fused kernel): the frame goes through in three bands of rows (whole tiles of four row pairs), one per
+    // stream, so the upload of band k + 1, the kernel of band k and the download of band k - 1 overlap -- the call is PCIe bound and
+    // PCIe is full duplex.
     // A band re-uploads the few chroma lines it shares with its neighbours (identical bytes), so bands need no cross-stream order.
-    if (c->route == R_FUSED && c->fast_ok && !nv && c->D->fam == FAM_RGB24 && !odd && tuning("sws_fused_variant") != 1 &&
-        tuning("sws_host_bands") != 1 && g.dstH >= 64 && !((uintptr_t)c->dev.vChrF & 15)) {
-        const int pairs = g.dstH / 2, nb = tuning("sws_host_bands") > 1 ? tuning("sws_host_bands") : 3, per = ((pairs + nb - 1) / nb + 3) & ~3;
+    if (c->route == R_FUSED && c->fast_ok && !nv && c->D->fam == FAM_RGB24 && !odd && g.dstH >= 64 && !((uintptr_t)c->dev.vChrF & 15)) {
+        const int pairs = g.dstH / 2, per = ((pairs + 2) / 3 + 3) & ~3;        // row pairs per band
         int k = 0;
         for (int rp0 = 0; rp0 < pairs; rp0 += per, k = (k + 1) % 3) {
             const int rp1 = rp0 + per < pairs ? rp0 + per : pairs, y0 = 2 * rp0, y1 = 2 * rp1;

@@ -51,20 +51,17 @@ __device__ __forceinline__ void tma_load_2d(unsigned dst_s, const CUtensorMap *t
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  :: "r"(dst_s), "l"(reinterpret_cast<uint64_t>(tm)), "r"(x), "r"(y), "r"(mbar_s) : "memory");
 }
-// shared -> global bulk tensor store (bulk async-group completion); the source must have been made visible with fence_proxy_async()
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap *tm, int x, int y, int z, unsigned src_s)
-{
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%1, %2, %3}], [%4];"
-                 :: "l"(reinterpret_cast<uint64_t>(tm)), "r"(x), "r"(y), "r"(z), "r"(src_s) : "memory");
-}
-// the same two operations with an L2 cache policy (createpolicy) attached to their global-memory side
+// an L2 cache policy (createpolicy) for the global-memory side of the two operations below
 __device__ __forceinline__ uint64_t l2_policy_evict_first()
 { uint64_t p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p; }
+// tma_load_3d with the policy attached
 __device__ __forceinline__ void tma_load_3d_hint(unsigned dst_s, const CUtensorMap *tm, int x, int y, int z, unsigned mbar_s, uint64_t policy)
 {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3, %4}], [%5], %6;"
                  :: "r"(dst_s), "l"(reinterpret_cast<uint64_t>(tm)), "r"(x), "r"(y), "r"(z), "r"(mbar_s), "l"(policy) : "memory");
 }
+// shared -> global bulk tensor store (bulk async-group completion) with the policy attached; the source must have been made visible
+// with fence_proxy_async()
 __device__ __forceinline__ void tma_store_3d_hint(const CUtensorMap *tm, int x, int y, int z, unsigned src_s, uint64_t policy)
 {
     asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group.L2::cache_hint [%0, {%1, %2, %3}], [%4], %5;"

@@ -1,12 +1,12 @@
 """The 8-bit H.264 batch calls against the reference on the edge cases of tests/h264_edge_cases.py, under every kernel the launchers can
-pick: the defaults, the fallbacks forced by their knobs (mc_variant = 2, residual_variant = 2) and reached by the inputs that need them,
-and both other register budgets of the MC kernel (mc_min_blocks 4 / 8).  Pictures sit in decoder layout inside poisoned allocations:
-besides the pixels and the consumed coefficient arena, every byte outside the picture rectangles must come back unchanged.
+pick: the defaults, and the fallbacks forced by their knobs (mc_variant = 2, residual_variant = 2) and reached by the inputs that need
+them.  Pictures sit in decoder layout inside poisoned allocations: besides the pixels and the consumed coefficient arena, every byte
+outside the picture rectangles must come back unchanged.
 
 The inputs that send a call to its fallback kernel (libav_b200/csrc):
-  MC        h264_mc.cu:119 luma plane or linesize not 4-byte aligned (pad2, shift1, shift2), :120 chroma plane or uvlinesize odd
-            (odd_uv, odd_cb), :121 odd pic_w / pic_h; inside the default kernel, a reference plane off 4-byte alignment sends every
-            block down the EDGE path (:74, ref1)
+  MC        h264_mc.cu:118 luma plane or linesize not 4-byte aligned (pad2, shift1, shift2), :119 chroma plane or uvlinesize odd
+            (odd_uv, odd_cb), :120 odd pic_w / pic_h; inside the default kernel, a reference plane off 4-byte alignment sends every
+            block down the EDGE path (:73, ref1)
   residual  h264_residual.cu:171 coeff_stride % 8 (772) or an arena off 16-byte alignment (+2 bytes), :172 planes or line sizes off
             4-byte alignment (pad2, shift1, shift2, odd_uv); coeff_stride 776 keeps the default kernel at a stride other than 768
   deblock   h264dsp.cu:274 refuses planes and line sizes off 4-byte alignment"""
@@ -23,7 +23,7 @@ import h264_util as hu
 pytestmark = pytest.mark.gpu
 MB_W, MB_H = 12, 8
 TIGHT = ec.Layout("tight", 0, 0)
-MC_KNOBS = [{}, {"mc_variant": 2}, {"mc_min_blocks": 4}, {"mc_min_blocks": 8}]
+MC_KNOBS = [{}, {"mc_variant": 2}]
 RES_KNOBS = [{}, {"residual_variant": 2}]
 knob_id = lambda k: ",".join("%s=%d" % kv for kv in k.items()) or "default"
 
@@ -103,7 +103,7 @@ def test_mc_any_record_order_and_batch_size(gpu, checker, mc_case, knobs):
         run_mc(gpu, sub, refs, dst, ec.PAD4, 16 * MB_W, 16 * MB_H, knobs).check(ec.oracle_mc(checker, sub, refs, dst), n)
 
 
-@pytest.mark.parametrize("knobs", MC_KNOBS[:2], ids=knob_id)
+@pytest.mark.parametrize("knobs", MC_KNOBS, ids=knob_id)
 def test_mc_stacked_pictures_far_vectors(gpu, checker, knobs):
     """two pictures stacked in one call, vectors up to the level limits in both directions: clamping stops at each picture's seam"""
     mb_w, mb_h, P = 6, 4, 2
