@@ -199,7 +199,13 @@ int ff_h264_dc_dequant_batch_422_cuda(const FFH264DCRecord *recs, size_t n, int1
  * ff_h264_idct_add_mb_batch_cuda (DC transforms already applied); consumed coefficients are zeroed like the C code.
  * Rows run as a wavefront two macroblocks behind the row above; progress = mb_h * n_pictures uint32 of scratch.
  * Pictures of a batch are stacked vertically (no prediction across a picture boundary; the records say what is
- * available).  Not covered: transform bypass (the lossless *_add predictors exist as table slots only), MBAFF. */
+ * available: the kernel follows topleft / topright_samples_available, not the picture geometry, so slices and
+ * constrained_intra_pred are expressed by the masks).  Not covered: transform bypass (the lossless *_add predictors exist
+ * as table slots only), MBAFF.
+ * Requirements (anything else returns -1 before any work is queued): no NULL pointer; mbs, nnzc and coeffs 4-byte
+ * aligned, coeff_stride even and >= 768 (each intra macroblock fetches and writes back the whole 768-element row, blocks
+ * 36..47 included, so a shorter stride would overlap the next macroblock's coefficients); luma / cb / cr, linesize and
+ * uvlinesize 4-byte aligned.  ff_h264_flush_pictures_cuda checks the same before its first stage when `intra` is set. */
 typedef struct FFH264IntraMB {
     uint8_t  kind;             /* 0 not intra, 1 intra 4x4, 2 intra 4x4 with the 8x8 transform (pred8x8l), 3 intra 16x16 */
     uint8_t  mode16;           /* sl->intra16x16_pred_mode (kind 3) */

@@ -28,6 +28,9 @@ int  check_launch(const char *where);   // cudaGetLastError() -> sticky error, r
 void enter();                   // make the device avb200_init() chose current in the calling thread (first statement of every public entry point)
 int sm_count();                 // multiprocessor count of the current device (cached)
 int tuning(const char *key);    // test knob set through avb200_set_tuning(); 0 when unset
+// the arguments the 8-bit intra wavefront needs (h264intra.cu); false = refused with a message.  mbs: const FFH264IntraMB *
+bool h264_intra_args_ok(const char *where, const void *mbs, const int16_t *coeffs, size_t coeff_stride, const uint8_t *nnzc, const uint8_t *luma,
+                        const uint8_t *cb, const uint8_t *cr, int linesize, int uvlinesize, const uint32_t *progress);
 
 // ---- device helpers ------------------------------------------------------------------------
 #ifdef AVB_HOSTSIM

@@ -531,6 +531,7 @@ static int launch_intra_generic(const char *where, int bit_depth, const FFH264In
                                 const uint8_t *nnzc, uint8_t *luma, uint8_t *cb, uint8_t *cr, int ls, int uvls, cudaStream_t st)
 {
     if (!mbs || !coeffs || !nnzc || !luma || !cb || !cr || mb_w <= 0 || mb_h <= 0 || n_pictures < 0 || mb_h > 8192) { set_error_msg(where, "bad argument"); return -1; }
+    if ((uintptr_t)coeffs % sizeof(typename Transform<PX>::coef)) { set_error_msg(where, "coeffs must be aligned to its coefficient type (int16 at 8 bit, int32 at 9 / 10)"); return -1; }
     if (!n_pictures) return 0;
     h264_intra_generic_kernel<PX, C422><<<(unsigned)n_pictures, DB_WARPS * 32, (size_t)mb_h * sizeof(int), st>>>(
         bit_depth, mbs, mb_w, mb_h, static_cast<typename Transform<PX>::coef *>(coeffs), coeff_stride, nnzc, luma, cb, cr, ls, uvls);

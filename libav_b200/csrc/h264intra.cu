@@ -268,6 +268,22 @@ h264_intra_kernel(const FFH264IntraMB *__restrict__ mbs, int mb_w, int rows_pp, 
     }
 }
 
+// What h264_intra_kernel needs of its arguments (the header comment of ff_h264_intra_mb_batch_cuda): the records, nnzc and every coefficient
+// row are fetched with 4-byte cp.async, the planes are read and written as words, and a macroblock fetches and writes back 768 coefficients
+bool h264_intra_args_ok(const char *where, const void *mbs, const int16_t *coeffs, size_t coeff_stride, const uint8_t *nnzc, const uint8_t *luma,
+                        const uint8_t *cb, const uint8_t *cr, int linesize, int uvlinesize, const uint32_t *progress)
+{
+    if (!mbs || !coeffs || !nnzc || !luma || !cb || !cr || !progress) { set_error_msg(where, "NULL argument"); return false; }
+    if ((linesize & 3) || (uvlinesize & 3) || ((uintptr_t)luma & 3) || ((uintptr_t)cb & 3) || ((uintptr_t)cr & 3)) {
+        set_error_msg(where, "planes and pitches must be 4-byte aligned"); return false;
+    }
+    if (((uintptr_t)mbs & 3) || ((uintptr_t)nnzc & 3) || ((uintptr_t)coeffs & 3) || (coeff_stride & 1)) {
+        set_error_msg(where, "mbs, nnzc and coeffs must be 4-byte aligned and coeff_stride even"); return false;
+    }
+    if (coeff_stride < 768) { set_error_msg(where, "coeff_stride must be at least 768"); return false; }
+    return true;
+}
+
 }  // namespace avb
 
 using namespace avb;
@@ -278,9 +294,7 @@ extern "C" int ff_h264_intra_mb_batch_cuda(const FFH264IntraMB *mbs, int mb_w, i
 {
     avb::enter();
     if (mb_w <= 0 || mb_h <= 0 || n_pictures <= 0) return 0;
-    if ((linesize & 3) || (uvlinesize & 3) || ((uintptr_t)luma & 3) || ((uintptr_t)cb & 3) || ((uintptr_t)cr & 3)) {
-        set_error_msg("ff_h264_intra_mb_batch_cuda", "planes and pitches must be 4-byte aligned"); return -1;
-    }
+    if (!h264_intra_args_ok("ff_h264_intra_mb_batch_cuda", mbs, coeffs, coeff_stride, nnzc, luma, cb, cr, linesize, uvlinesize, progress)) return -1;
     cudaStream_t st = (cudaStream_t)stream;
     const int rows = mb_h * n_pictures;
     AVB_CUDA(cudaMemsetAsync(progress, 0, sizeof(uint32_t) * rows, st), "ff_h264_intra_mb_batch_cuda");

@@ -296,6 +296,9 @@ extern "C" int ff_h264_flush_pictures_cuda(const FFH264PictureWork *w, void *str
         }
         return 0;
     }
+    // an intra arena stage 5 would refuse is refused before stage 1 writes anything
+    if (w->intra && !h264_intra_args_ok("ff_h264_flush_pictures_cuda", w->intra, w->coeffs, w->coeff_stride, w->nnzc, w->luma, w->cb, w->cr,
+                                        w->linesize, w->uvlinesize, w->progress)) return -1;
     // 1. inter prediction: every put partition, then every avg partition (h264_mb.c:322-366)
     if (w->n_mc && ff_h264_mc_batch_cuda(w->mc, w->n_mc, w->refs, w->luma, w->cb, w->cr, w->linesize, w->uvlinesize, 16 * w->mb_w, 16 * w->mb_h, stream)) return -1;
     // 2. explicit / implicit weighted prediction on the predicted blocks (h264_mb.c:368-460), plane by plane

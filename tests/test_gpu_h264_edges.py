@@ -226,24 +226,15 @@ def test_deblock_refuses_unaligned_planes(gpu, lay):
 
 
 # ---- the flush point in decoder layout ----
-def test_flush_in_decoder_layout(gpu, checker):
-    """ff_h264_flush_pictures_cuda over two stacked pictures whose planes have line sizes wider than the picture: every stage's
-    records address the decoder's layout, the checker runs on tight copies"""
+def flush_batch(works, pics, refs, mb_w, mb_h, lay=ec.PAD4):
+    """works (test_gpu_h264flush.picture_work) and their pictures stacked into one FFH264PictureWork, planes and reference planes placed
+    by `lay`: returns (work, placed pictures, the device buffers work points to)"""
     from libav_b200 import device
-    from test_gpu_h264flush import picture_work, oracle_chain
-    mb_w, mb_h, P = 20, 12, 2
+    P = len(works)
     W, H = 16 * mb_w, 16 * mb_h
-    refs = [synth.h264_picture(mb_w, mb_h, seed=11), synth.h264_picture(mb_w, mb_h, seed=12)]
-    works = [picture_work(mb_w, mb_h, 300 + 100 * k, 0.25) for k in range(P)]
-    pics = [synth.h264_picture(mb_w, mb_h, seed=70 + k) for k in range(P)]
-    want, want_co = [], []
-    for w, p in zip(works, pics):
-        wp = [x.copy() for x in p]
-        want_co.append(oracle_chain(checker, w, refs, mb_w, mb_h, *wp))
-        want.append(wp)
     cat = lambda planes: [np.concatenate([p[i] for p in planes]) for i in range(3)]
-    d = Placed(ec.PAD4, cat(pics))
-    r = [Placed(ec.PAD4, [np.concatenate([p] * P) for p in rp], ref=True) for rp in refs]
+    d = Placed(lay, cat(pics))
+    r = [Placed(lay, [np.concatenate([p] * P) for p in rp], ref=True) for rp in refs]
     ls, uvls = d.ls[0], d.ls[1]
     mc, res, wrec = [], [], []
     for k, w in enumerate(works):
@@ -262,7 +253,7 @@ def test_flush_in_decoder_layout(gpu, checker):
     catw = lambda k: np.concatenate([w[k] for w in works])
     dv = dict(planes=_dev(np.array([p.ptrs for p in r], np.uint64)), mc=_dev(mc), res=_dev(res), w=_dev(wrec), co=_dev(catw("coeffs")),
               nz=_dev(catw("nnzc")), dc=_dev(catw("dc")), ldc=_dev(catw("luma_dc")), intra=_dev(catw("intra")), rec=device.DevBuf(n * 104),
-              prog=device.DevBuf(4 * 2 * mb_h * P))
+              prog=device.DevBuf(4 * 2 * mb_h * P), keep=keep, info=info, refs=r)
     work = tables.FFH264PictureWork()
     work.mb_w, work.mb_h, work.n_pictures = mb_w, mb_h, P
     work.luma, work.cb, work.cr = d.ptrs
@@ -272,8 +263,25 @@ def test_flush_in_decoder_layout(gpu, checker):
     work.coeffs, work.coeff_stride, work.nnzc = dv["co"].ptr, 768, dv["nz"].ptr
     work.dc, work.luma_dc, work.residual, work.intra = dv["dc"].ptr, dv["ldc"].ptr, dv["res"].ptr, dv["intra"].ptr
     work.deblock_info, work.deblock_records, work.progress = C.pointer(info), dv["rec"].ptr, dv["prog"].ptr
+    return work, d, dv
+
+
+def test_flush_in_decoder_layout(gpu, checker):
+    """ff_h264_flush_pictures_cuda over two stacked pictures whose planes have line sizes wider than the picture: every stage's
+    records address the decoder's layout, the checker runs on tight copies"""
+    from libav_b200 import device
+    from test_gpu_h264flush import picture_work, oracle_chain
+    mb_w, mb_h, P = 20, 12, 2
+    refs = [synth.h264_picture(mb_w, mb_h, seed=11), synth.h264_picture(mb_w, mb_h, seed=12)]
+    works = [picture_work(mb_w, mb_h, 300 + 100 * k, 0.25) for k in range(P)]
+    pics = [synth.h264_picture(mb_w, mb_h, seed=70 + k) for k in range(P)]
+    want, want_co = [], []
+    for w, p in zip(works, pics):
+        wp = [x.copy() for x in p]
+        want_co.append(oracle_chain(checker, w, refs, mb_w, mb_h, *wp))
+        want.append(wp)
+    work, d, dv = flush_batch(works, pics, refs, mb_w, mb_h)
     gpu.check(gpu.lib.ff_h264_flush_pictures_cuda(C.byref(work), None))
     device.sync()
-    d.check(cat(want))
-    assert np.array_equal(dv["co"].download(np.int16, (n, 768)), np.concatenate(want_co))
-
+    d.check([np.concatenate([w[i] for w in want]) for i in range(3)])
+    assert np.array_equal(dv["co"].download(np.int16, (mb_w * mb_h * P, 768)), np.concatenate(want_co))
