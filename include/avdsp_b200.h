@@ -324,9 +324,13 @@ int ff_h264_deblock_batch_422_cuda(int bit_depth, const FFH264DeblockMB *mbs, co
 
 /* Deblocking DECISIONS (SURVEY 8f rank 1): what loop_filter() -> fill_filter_caches() -> ff_h264_filter_mb()
  * (libavcodec/h264_slice.c:1972-2262, libavcodec/h264_loopfilter.c:438-846) decide for every macroblock of a
- * progressive 4:2:0 8-bit picture -- boundary strengths, averaged qp, alpha / beta / tc0 per edge -- computed on the
+ * progressive picture -- boundary strengths, averaged qp, alpha / beta / tc0 per edge -- computed on the
  * device from the decoder's side-information arrays, written as the FFH264DeblockMB records the deblocking kernels
- * above consume.  All pointers are DEVICE pointers to copies of the decoder's own arrays, in the decoder's layouts:
+ * above consume.  ff_h264_deblock_params_cuda decides for 8-bit pictures; ff_h264_deblock_params_hbd_cuda takes the bit depth
+ * (8, 9 or 10; 8 gives exactly what ff_h264_deblock_params_cuda gives, any other is refused and `out` left untouched).  At 9 / 10 bit
+ * qscale_table and chroma_qp_table are the decoder's, in the QP' scale (0..51 + 6 * (bit_depth - 8); I_PCM macroblocks hold 0), and
+ * qp_thresh carries its + 6 * (bit_depth - 8) term; the records still hold the 8-bit-scale alpha / beta / tc0 of the reference's tables
+ * (h264_loopfilter.c:256-258,726-728), which ff_h264_deblock_batch_hbd_cuda / ff_h264_deblock_batch_422_cuda scale.  All pointers are DEVICE pointers to copies of the decoder's own arrays, in the decoder's layouts:
  *   mb_type, qscale_table, cbp_table, slice_table: [n_pictures * mb_h][mb_w + 1] (mb_stride = mb_w + 1, the extra
  *       column is the decoder's padding and is never read)          H264Picture.mb_type / qscale_table, H264Context
  *   non_zero_count: [..][48] per macroblock                          H264Context.non_zero_count
@@ -364,6 +368,7 @@ typedef struct FFH264DeblockInfo {
                                                macroblock m are written to chroma422[m] instead of the 104-byte record's [plane][1][..] */
 } FFH264DeblockInfo;
 int ff_h264_deblock_params_cuda(const FFH264DeblockInfo *info /* host struct */, FFH264DeblockMB *out, void *stream);
+int ff_h264_deblock_params_hbd_cuda(int bit_depth, const FFH264DeblockInfo *info /* host struct */, FFH264DeblockMB *out, void *stream);
 
 /* The flush point of a decoder back-end (SURVEY 8f rank 1): the CPU parses and entropy-decodes, RECORDS the work of a batch of
  * pictures (or of the slices decoded so far) in the arrays below, and flushes it with one call.  The stages run on `stream` in
@@ -393,7 +398,8 @@ typedef struct FFH264PictureWork {
     uint32_t *progress;
     int bit_depth, chroma_format_idc;        /* 0 = 8 / 1.  9 / 10-bit pictures (int32 coeffs / luma_dc behind the same pointers) and 4:2:2 chroma at
                                                 8 / 9 / 10 bit run the *_hbd_cuda / *_422_cuda stages in the same order (progress is not used then;
-                                                4:2:2 intra macroblocks: ff_h264_intra_mb_batch_422_cuda) */
+                                                4:2:2 intra macroblocks: ff_h264_intra_mb_batch_422_cuda; decisions from deblock_info:
+                                                ff_h264_deblock_params_hbd_cuda at bit_depth, so its side information is in the QP' scale) */
     const FFH264DeblockChroma422 *deblock_chroma422;   /* 4:2:2 with caller-filled deblock_records: their second record array */
 } FFH264PictureWork;
 int ff_h264_flush_pictures_cuda(const FFH264PictureWork *work /* host struct */, void *stream);

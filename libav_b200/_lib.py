@@ -70,6 +70,7 @@ PROTOTYPES = {
     "ff_h264_deblock_picture_cuda": (i32, [vp, i32, i32, vp, vp, vp, i32, i32, vp, vp]),
     "ff_h264_deblock_batch_cuda": (i32, [vp, i32, i32, i32, vp, vp, vp, i32, i32, vp, vp]),
     "ff_h264_deblock_params_cuda": (i32, [vp, vp, vp]),
+    "ff_h264_deblock_params_hbd_cuda": (i32, [i32, vp, vp, vp]),
     "ff_h264_flush_pictures_cuda": (i32, [vp, vp]),
     "ff_h264_dc_dequant_batch_cuda": (i32, [vp, sz, vp, sz, vp, vp]),
     "ff_h264_dc_dequant_batch_422_cuda": (i32, [vp, sz, vp, sz, vp, vp]),

@@ -1,7 +1,7 @@
 // libav_b200/csrc/h264lf.cu -- H.264 deblocking DECISIONS on the device (SURVEY 8f rank 1).
 //
 // Replaces the per-macroblock scalar walk loop_filter() -> fill_filter_caches() -> ff_h264_filter_mb()
-// (libavcodec/h264_slice.c:1972-2262, libavcodec/h264_loopfilter.c:438-846) for progressive 4:2:0 8-bit pictures:
+// (libavcodec/h264_slice.c:1972-2262, libavcodec/h264_loopfilter.c:438-846) for progressive 4:2:0 / 4:2:2 pictures of 8, 9 or 10 bit:
 // from the decoder's side-information arrays (device copies, the decoder's own layouts) it writes one FFH264DeblockMB
 // per macroblock -- the (alpha, beta, tc0 | bS 4) of every edge -- which ff_h264_deblock_batch_cuda consumes without
 // a host round trip.  One thread = one (macroblock, direction): it owns every field of the record indexed by that
@@ -32,6 +32,7 @@ struct Blk { int nz, ref0, ref1; int mv0, mv1; };          // mv = packed (x, y)
 struct LfPic {
     FFH264DeblockInfo i;
     int ms, bs;
+    int qp_bd_offset;           // 6 * (bit_depth - 8): qscale_table / chroma_qp_table hold QP', the threshold tables are indexed by QP
 };
 
 // the 4x4 block (bx, by) of macroblock xy (picture-stacked index) as the loop filter sees it; `type` = macroblock
@@ -136,7 +137,9 @@ h264_deblock_params_kernel(LfPic p, FFH264DeblockMB *__restrict__ out, int n_mbs
         const int nxy = dir ? xy - p.ms : xy - 1;
         uint32_t mt = (dir ? y > 0 : x > 0) ? p.i.mb_type[nxy] : 0;
         if (mt && sl.deblocking_filter == 2 && p.i.slice_table[nxy] != sn) mt = 0;
-        const int offa = sl.alpha_c0_offset, offb = sl.beta_offset, lists = sl.list_count;
+        // the offsets reach only the table index: the reference's a = 52 + offset - qp_bd_offset (h264_loopfilter.c:256-258,726-728); the
+        // qp averaging and the low-qp shortcut stay in QP'
+        const int offa = sl.alpha_c0_offset - p.qp_bd_offset, offb = sl.beta_offset - p.qp_bd_offset, lists = sl.list_count;
         const int mask_edge = dir ? (0x33331130u >> (4 * ((type >> 3) & 7))) & 15 : (0x11113330u >> (4 * ((type >> 3) & 7))) & 15;
         const bool is_intra = type & T_INTRA;
         const int edges = (mask_edge == 3 && !is_intra && !(p.i.cbp_table[xy] & 15)) ? 1 : 4;
@@ -238,17 +241,28 @@ h264_deblock_params_kernel(LfPic p, FFH264DeblockMB *__restrict__ out, int n_mbs
 
 using namespace avb;
 
-extern "C" int ff_h264_deblock_params_cuda(const FFH264DeblockInfo *info, FFH264DeblockMB *out, void *stream)
+static int deblock_params(const char *fn, int bit_depth, const FFH264DeblockInfo *info, FFH264DeblockMB *out, void *stream)
 {
     avb::enter();
+    if (bit_depth != 8 && bit_depth != 9 && bit_depth != 10) { set_error_msg(fn, "bit_depth 8 / 9 / 10"); return -1; }
     if (!info || !out || info->mb_w <= 0 || info->mb_h <= 0 || info->n_pictures <= 0 || info->n_slices <= 0 || info->n_slices > 32) {
-        set_error_msg("ff_h264_deblock_params_cuda", "bad arguments (1..32 slices per call: the reference keeps 32 ref2frm tables)");
+        set_error_msg(fn, "bad arguments (1..32 slices per call: the reference keeps 32 ref2frm tables)");
         return -1;
     }
-    LfPic p; p.i = *info; p.ms = info->mb_w + 1; p.bs = 4 * info->mb_w;
+    LfPic p; p.i = *info; p.ms = info->mb_w + 1; p.bs = 4 * info->mb_w; p.qp_bd_offset = 6 * (bit_depth - 8);
     const int n = info->mb_w * info->mb_h * info->n_pictures;
     h264_deblock_params_kernel<<<(2 * n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(p, out, n);
-    return check_launch("ff_h264_deblock_params_cuda");
+    return check_launch(fn);
+}
+
+extern "C" int ff_h264_deblock_params_cuda(const FFH264DeblockInfo *info, FFH264DeblockMB *out, void *stream)
+{
+    return deblock_params("ff_h264_deblock_params_cuda", 8, info, out, stream);
+}
+
+extern "C" int ff_h264_deblock_params_hbd_cuda(int bit_depth, const FFH264DeblockInfo *info, FFH264DeblockMB *out, void *stream)
+{
+    return deblock_params("ff_h264_deblock_params_hbd_cuda", bit_depth, info, out, stream);
 }
 
 // The decoder back-end's flush point (SURVEY 8f rank 1): everything the CPU recorded for a batch of pictures / slices, run in the
@@ -286,7 +300,7 @@ extern "C" int ff_h264_flush_pictures_cuda(const FFH264PictureWork *w, void *str
                 (idc == 2) != (w->deblock_info->chroma422 != nullptr)) {
                 set_error_msg("ff_h264_flush_pictures_cuda", "deblock_info does not describe this batch"); return -1;
             }
-            if (ff_h264_deblock_params_cuda(w->deblock_info, w->deblock_records, stream)) return -1;
+            if (ff_h264_deblock_params_hbd_cuda(depth, w->deblock_info, w->deblock_records, stream)) return -1;
         }
         if (w->deblock_records) {
             if (idc == 2) {

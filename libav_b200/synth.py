@@ -297,17 +297,34 @@ def h264_deblock_work(mb_w, mb_h, seed=4, slices=1):
 
 
 # ---- decoder side information for the deblocking-decision kernel (the reference's own array layouts) ----
-MB_INTRA4x4, MB_INTRA16x16, MB_16x16, MB_16x8, MB_8x16, MB_8x8 = 1, 2, 8, 16, 32, 64
+MB_INTRA4x4, MB_INTRA16x16, MB_INTRA_PCM, MB_16x16, MB_16x8, MB_8x16, MB_8x8 = 1, 2, 4, 8, 16, 32, 64
 MB_DIRECT2, MB_SKIP, MB_P0L0, MB_P1L0, MB_P0L1, MB_P1L1, MB_8x8DCT = 0x100, 0x800, 0x1000, 0x2000, 0x4000, 0x8000, 0x01000000
 H264_CHROMA_QP = np.array(list(range(30)) + [29, 30, 31, 32, 32, 33, 34, 34, 35, 35, 36, 36, 37, 37, 37, 38, 38, 38, 39, 39, 39, 39], np.uint8)
 
 
+def h264_chroma_qp_table(bit_depth, offset):
+    """One row of PPS.chroma_qp_table in the decoder's QP' scale: QP'c for QP'y = 0..max_qp (max_qp = 51 + qp_bd_offset) and
+    chroma_qp_index_offset `offset`.  The standard's qPI = Clip3(-QpBdOffsetC, 51, QPy + offset) maps to QPc through H264_CHROMA_QP
+    (identity below 30, so also for the negative qPI of 9 / 10 bit), and QP'c = QPc + QpBdOffsetC.  Entries past max_qp stay 0."""
+    bd = 6 * (bit_depth - 8)
+    max_qp = 51 + bd
+    qpi = np.clip(np.arange(max_qp + 1) + offset, 0, max_qp) - bd
+    row = np.zeros(64, np.uint8)
+    row[:max_qp + 1] = np.where(qpi < 0, qpi, H264_CHROMA_QP[np.maximum(qpi, 0)]) + bd
+    return row
+
+
 def h264_deblock_info(mb_w, mb_h, seed=5, n_slices=3, bipred=False, cabac=1, t8x8=0, mode=1, qp_lo=10, qp_hi=51,
-                      p_intra=0.15, cb_off=0, cr_off=0):
+                      p_intra=0.15, cb_off=0, cr_off=0, bit_depth=8):
     """Random but self-consistent side information of one progressive picture, in the layouts libavcodec keeps it
     (H264Picture.mb_type / qscale_table / motion_val / ref_index, H264Context.non_zero_count / cbp_table /
     slice_table / ref2frm, PPS.chroma_qp_table): what ff_h264_deblock_params_cuda and the oracle consume.
-    Motion vectors differ by 0..8 quarter-pels between partitions so the |d| >= 4 rule is exercised both ways."""
+    Motion vectors differ by 0..8 quarter-pels between partitions so the |d| >= 4 rule is exercised both ways.
+    bit_depth 9 / 10: qscale_table, chroma_qp_table and qp_thresh in the decoder's QP' scale (0..max_qp, max_qp = 51 + 6 * (bit_depth - 8),
+    h264_cavlc.c:1094, h264_ps.c:662, h264_slice.c:1815-1820), drawn from a second random stream after the 8-bit draws: qscale weighted
+    towards both ends -- 0 (some of those macroblocks I_PCM, which the decoder stores with qscale 0, h264_cavlc.c:782), the slice's
+    qp_thresh +- 2 and max_qp -- and otherwise uniform over [qp_lo, qp_hi] + qp_bd_offset; alpha / beta offsets over -12..12; unless
+    cb_off / cr_off are given, two different chroma_qp_index_offsets in -12..12."""
     r = np.random.RandomState(seed)
     ms, bs = mb_w + 1, 4 * mb_w
     n = ms * mb_h
@@ -376,10 +393,36 @@ def h264_deblock_info(mb_w, mb_h, seed=5, n_slices=3, bipred=False, cabac=1, t8x
                 r2f[l, 2 + i] = 4 * int(ids[(i + 2 * l) % 4 if bipred else i % 3]) + 3      # some indices share a frame
         sp[s, :5] = [a, b, mode, 2 if bipred else 1, 15 - min(a, b) - max(0, cb_off, cr_off)]
         sp[s, 5:] = r2f.reshape(-1)
+    if bit_depth != 8:
+        if bit_depth not in (9, 10):
+            raise ValueError("bit_depth 8, 9 or 10")
+        h = np.random.RandomState(seed + 1000 * bit_depth)
+        bd = 6 * (bit_depth - 8)
+        max_qp = 51 + bd
+        if cb_off == 0 and cr_off == 0:
+            cb_off, cr_off = (int(v) for v in h.choice(np.arange(-12, 13), 2, replace=False))
+        for s in range(n_slices):
+            a, b = 2 * h.randint(-6, 7), 2 * h.randint(-6, 7)
+            sp[s, :5] = [a, b, mode, 2 if bipred else 1, 15 - min(a, b) - max(0, cb_off, cr_off) + bd]
+        for y in range(mb_h):
+            for x in range(mb_w):
+                xy = x + y * ms
+                u = h.rand()
+                if u < 0.1:
+                    qp[xy] = 0
+                    if h.rand() < 0.5:
+                        mb_type[xy] = MB_INTRA_PCM
+                        nnz[xy] = 16
+                elif u < 0.2:
+                    qp[xy] = max_qp
+                elif u < 0.45:
+                    qp[xy] = np.clip(sp[sl[xy], 4] + h.randint(-2, 3), 0, max_qp)
+                else:
+                    qp[xy] = h.randint(min(qp_lo + bd, max_qp), min(qp_hi + bd, max_qp) + 1)
     cqt = np.zeros((2, 64), np.uint8)
     for t, off in enumerate((cb_off, cr_off)):
-        cqt[t, :52] = H264_CHROMA_QP[np.clip(np.arange(52) + off, 0, 51)]
-    d.update(mb_type=mb_type, qscale=qp, nnz=nnz, cbp=cbp, slice_table=sl, mv0=np.ascontiguousarray(mv[0]), mv1=np.ascontiguousarray(mv[1]),
+        cqt[t] = h264_chroma_qp_table(bit_depth, off)
+    d.update(bit_depth=bit_depth, mb_type=mb_type, qscale=qp, nnz=nnz, cbp=cbp, slice_table=sl, mv0=np.ascontiguousarray(mv[0]), mv1=np.ascontiguousarray(mv[1]),
              ref0=np.ascontiguousarray(ref[0]), ref1=np.ascontiguousarray(ref[1]), slice_params=sp, chroma_qp_table=cqt)
     return d
 

@@ -62,7 +62,9 @@ API = {
     "h264_deblock_picture_structure": (None, [i32]),
     "h264_deblock_chroma422": (None, [vp]),
     "h264_deblock_params": (i32, [i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, i32, vp]),
+    "h264_deblock_params_hbd": (i32, [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, i32, vp]),
     "h264_deblock_picture_with": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, i32]),
+    "h264_deblock_picture_with_hbd": (i32, [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, i32]),
     "h264_pictures": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32]),
     "me_cmp_select": (None, [vp, i32, vp]),
     "table_fill": (i32, [i32, i32, i32, vp, i32]),

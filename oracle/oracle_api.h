@@ -122,7 +122,7 @@ int ORC(me_cmp_quant)(int kind, int sidx, const OrcEncState *st, uint8_t *b1, ui
  * s->intra_scantable.scantable (the order the quantiser walks) */
 void ORC(enc_qmatrices)(const OrcEncState *st, int32_t *q_intra, int32_t *q_inter, uint8_t *scantable);
 
-/* Deblocking DECISIONS for one progressive 4:2:0 8-bit picture (SURVEY 8f rank 1): what loop_filter() ->
+/* Deblocking DECISIONS for one progressive 4:2:0 8-bit picture (SURVEY 8f rank 1; h264_deblock_params_hbd: of bit_depth 8, 9 or 10): what loop_filter() ->
  * fill_filter_caches() -> ff_h264_filter_mb() (libavcodec/h264_slice.c:2198-2262, :1972-2196,
  * libavcodec/h264_loopfilter.c:420-846) decide per macroblock -- which edges are filtered with which
  * (alpha, beta, tc0 | bS 4).  Inputs are the decoder's own side-information arrays in the decoder's layouts:
@@ -134,13 +134,19 @@ void ORC(enc_qmatrices)(const OrcEncState *st, int32_t *q_intra, int32_t *q_inte
  *   slice_params: per slice_num 133 int32 = { slice_alpha_c0_offset, slice_beta_offset, deblocking_filter,
  *                 list_count, qp_thresh, ref2frm[2][64] }  (H264SliceContext / H264Context.ref2frm, h264dec.h:186,538)
  *   chroma_qp_table: PPS.chroma_qp_table[2][64] (h264_ps.h:124)
+ * At 9 / 10 bit qscale and chroma_qp_table are in the decoder's QP' scale (0..51 + 6 * (bit_depth - 8)), and qp_thresh carries its
+ * + 6 * (bit_depth - 8) term (h264_slice.c:1815-1820); the records keep the 8-bit-scale alpha / beta / tc0 the filters are called with.
  * out: mb_w * mb_h records of 104 bytes, raster order, in the layout of FFH264DeblockMB (include/avdsp_b200.h):
  *   alpha[2][4] beta[2][4] tc0[2][4][4] intra[2] calpha[2][2][2] cbeta[2][2][2] ctc0[2][2][2][4] cintra[2][2] pad[2];
- *   an edge that is not filtered has alpha = beta = 0. Returns 0, or -1 for n_slices > 32. */
+ *   an edge that is not filtered has alpha = beta = 0. Returns 0, or -1 for n_slices > 32 or a bit_depth other than 8 / 9 / 10. */
 int ORC(h264_deblock_params)(int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
                              const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
                              const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
                              const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out);
+int ORC(h264_deblock_params_hbd)(int bit_depth, int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
+                                 const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
+                                 const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
+                                 const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out);
 /* the pictures of the following h264_deblock_params / h264_deblock_picture_with calls are fields (h->picture_structure != PICT_FRAME; their
  * mb_type entries must carry MB_TYPE_INTERLACED, 0x80): mvy_limit 2, bS 3 on horizontal intra macroblock edges (h264_loopfilter.c:551-557,723) */
 void ORC(h264_deblock_picture_structure)(int field_picture);

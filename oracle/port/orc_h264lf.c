@@ -1,7 +1,7 @@
 /*
  * oracle/port/orc_h264lf.c -- TEST INFRASTRUCTURE, NOT PRODUCT.
  *
- * CPU restatement of the H.264 deblocking DECISIONS for progressive 4:2:0 8-bit pictures: boundary strength per
+ * CPU restatement of the H.264 deblocking DECISIONS for progressive 4:2:0 / 4:2:2 pictures at 8, 9 or 10 bit: boundary strength per
  * 4-sample edge segment and the (alpha, beta, tc0) each edge is filtered with, i.e. what
  *   loop_filter() / fill_filter_caches()           libavcodec/h264_slice.c:1972-2262
  *   ff_h264_filter_mb() / filter_mb_dir() / check_mv()  libavcodec/h264_loopfilter.c:438-846
@@ -9,7 +9,9 @@
  * hand to the H264DSPContext loop-filter slots.  Written from the picture-level arrays directly (no per-macroblock
  * caches): strength(dir, edge, i) looks the two 4x4 blocks of segment i up where they live.  The threshold tables
  * are the standard's alpha'/beta'/tC0' with the index clipped to 0..51, which is what the reference's zero-/
- * constant-padded tables (:40-101) evaluate to.  Pinned byte-for-byte against oracle/_ref (the reference's own
+ * constant-padded tables (:40-101) evaluate to.  At 9 / 10 bit qscale_table and chroma_qp_table hold QP' (0..51 + qp_bd_offset, the
+ * decoder's scale); only the table index subtracts qp_bd_offset = 6 * (bit_depth - 8) (:256-258,726-728), the qp averaging and the
+ * low-qp shortcut stay in QP'.  Pinned byte-for-byte against oracle/_ref (the reference's own
  * h264_loopfilter.c with recording slots) in tests/test_oracle_h264lf_cpu.py.
  */
 #include <stdint.h>
@@ -132,15 +134,16 @@ static void emit422(uint8_t *ext, int plane, int e, const int bS[4], int qp, int
         ext[48 + plane] |= 1 << e;
 }
 
-int orc_h264_deblock_params(int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
-                            const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
-                            const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
-                            const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out)
+int orc_h264_deblock_params_hbd(int bit_depth, int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
+                                const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
+                                const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
+                                const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out)
 {
     static const uint8_t mask_edge_tab[2][8] = { { 0, 3, 3, 3, 1, 1, 1, 1 }, { 0, 3, 1, 1, 3, 3, 3, 3 } };
     Pic p = { mb_w, mb_h, mb_w + 1, 4 * mb_w, cabac, transform_8x8_mode, mb_type, qscale, nnz, cbp, slice_table,
               { mv0, mv1 }, { ref0, ref1 }, slice_params, chroma_qp_table };
-    if (n_slices > 32) return -1;
+    if (n_slices > 32 || bit_depth < 8 || bit_depth > 10) return -1;
+    const int qp_bd_offset = 6 * (bit_depth - 8);
     memset(out, 0, (size_t)104 * mb_w * mb_h);
     if (g_ext422) memset(g_ext422, 0, (size_t)52 * mb_w * mb_h);
     for (int y = 0; y < mb_h; y++)
@@ -148,7 +151,8 @@ int orc_h264_deblock_params(int mb_w, int mb_h, const uint32_t *mb_type, const i
             const int xy = x + y * p.ms, sn = slice_table[xy];
             uint8_t *ext = g_ext422 ? g_ext422 + (size_t)52 * (x + y * mb_w) : NULL;
             const int32_t *sp = slice_params + 133 * sn;
-            const int offa = sp[0], offb = sp[1], mode = sp[2], lists = sp[3], th = sp[4];
+            /* offa / offb reach only the table index inside emit / emit422: the reference's a = 52 + offset - qp_bd_offset */
+            const int offa = sp[0] - qp_bd_offset, offb = sp[1] - qp_bd_offset, mode = sp[2], lists = sp[3], th = sp[4];
             const uint32_t type = mb_type[xy];
             const int qp = qscale[xy];
             uint8_t *rec = out + (size_t)104 * (x + y * mb_w);
@@ -221,4 +225,13 @@ int orc_h264_deblock_params(int mb_w, int mb_h, const uint32_t *mb_type, const i
             }
         }
     return 0;
+}
+
+int orc_h264_deblock_params(int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
+                            const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
+                            const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
+                            const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out)
+{
+    return orc_h264_deblock_params_hbd(8, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1, slice_params, n_slices,
+                                       chroma_qp_table, cabac, transform_8x8_mode, out);
 }

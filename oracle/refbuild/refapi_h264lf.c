@@ -1,7 +1,7 @@
 /*
  * oracle/refbuild/refapi_h264lf.c -- TEST INFRASTRUCTURE, NOT PRODUCT.
  *
- * ref_h264_deblock_params(): the reference's own deblocking DECISIONS for one picture.  The decision code is the
+ * ref_h264_deblock_params(): the reference's own deblocking DECISIONS for one picture, at bit depth 8, 9 or 10.  The decision code is the
  * unmodified libavcodec/h264_loopfilter.c (ff_h264_filter_mb_fast -> ff_h264_filter_mb, :420-437, :716-846), compiled
  * from /root/reference.  It is driven the way loop_filter() drives it (h264_slice.c:2198-2262): for each macroblock in
  * raster order fill the slice context's neighbour caches, set sl->chroma_qp[], call ff_h264_filter_mb_fast().  The
@@ -172,7 +172,7 @@ static int run_driver(const H264DSPContext *table, uint8_t *Y, uint8_t *Cb, uint
                       int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
                       const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
                       const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
-                      const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out)
+                      const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, int bit_depth, uint8_t *out)
 {
     const int ms = mb_w + 1, pad = 2 * ms + 1, n = ms * mb_h;
     H264Context *h = calloc(1, sizeof(*h));
@@ -210,7 +210,10 @@ static int run_driver(const H264DSPContext *table, uint8_t *Y, uint8_t *Cb, uint
     pps->cabac = cabac; pps->transform_8x8_mode = transform_8x8_mode;
     memcpy(pps->chroma_qp_table, chroma_qp_table, 128);
     pps->chroma_qp_diff = memcmp(chroma_qp_table, chroma_qp_table + 64, 64) != 0;
-    sps->bit_depth_luma = 8; sps->chroma_format_idc = (g_ext422 && !table) ? 2 : 1;
+    /* bit_depth_luma sets qp_bd_offset (h264_loopfilter.c:256,726); the recorders keep pixel_shift 0, so offsets into the fake planes still
+     * name the edge, while real 9 / 10-bit planes hold 16-bit samples */
+    sps->bit_depth_luma = bit_depth; sps->chroma_format_idc = (g_ext422 && !table) ? 2 : 1;
+    h->pixel_shift = table && bit_depth > 8;
     h->ps.pps = pps; h->ps.sps = sps;
     for (s = 0; s < n_slices; s++)
         memcpy(h->ref2frm[s], slice_params + 133 * s + 5, sizeof(h->ref2frm[s]));
@@ -236,7 +239,8 @@ static int run_driver(const H264DSPContext *table, uint8_t *Y, uint8_t *Cb, uint
                 continue;
             sl->chroma_qp[0] = pps->chroma_qp_table[0][h->cur_pic.qscale_table[xy] & 63];
             sl->chroma_qp[1] = pps->chroma_qp_table[1][h->cur_pic.qscale_table[xy] & 63];
-            if (table) ff_h264_filter_mb_fast(h, sl, x, y, Y + 16 * (x + (size_t)y * ls), Cb + 8 * (x + (size_t)y * uvls), Cr + 8 * (x + (size_t)y * uvls), ls, uvls);
+            if (table) ff_h264_filter_mb_fast(h, sl, x, y, Y + (16 * x << h->pixel_shift) + 16 * (size_t)y * ls, Cb + (8 * x << h->pixel_shift) + 8 * (size_t)y * uvls,
+                                              Cr + (8 * x << h->pixel_shift) + 8 * (size_t)y * uvls, ls, uvls);
             else       ff_h264_filter_mb_fast(h, sl, x, y, fake_y, fake_cb, fake_cr, REC_LS, REC_UVLS);
         }
     for (l = 0; l < 2; l++) free(t_ref[l]);
@@ -244,26 +248,49 @@ static int run_driver(const H264DSPContext *table, uint8_t *Y, uint8_t *Cb, uint
     return 0;
 }
 
+/* bit_depth 8 / 9 / 10 (-1 otherwise); ref_h264_deblock_params keeps its 8-bit signature */
+int ref_h264_deblock_params_hbd(int bit_depth, int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
+                                const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
+                                const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
+                                const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out)
+{
+    if (bit_depth < 8 || bit_depth > 10) return -1;
+    return run_driver(NULL, NULL, NULL, NULL, 0, 0, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1, slice_params, n_slices,
+                      chroma_qp_table, cabac, transform_8x8_mode, bit_depth, out);
+}
+
 int ref_h264_deblock_params(int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
                             const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
                             const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
                             const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode, uint8_t *out)
 {
-    return run_driver(NULL, NULL, NULL, NULL, 0, 0, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1, slice_params, n_slices,
-                      chroma_qp_table, cabac, transform_8x8_mode, out);
+    return ref_h264_deblock_params_hbd(8, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1, slice_params, n_slices,
+                                       chroma_qp_table, cabac, transform_8x8_mode, out);
 }
 
 /* The reference's own deblocking driver (ff_h264_filter_mb_fast -> ff_h264_filter_mb, raster order like loop_filter()) filtering a real
- * picture in place through the loop-filter entries of `table` -- an H264DSPContext filled by anybody: NULL = ff_h264dsp_init(8, 1), the
- * reference's C functions; otherwise e.g. the table ff_h264dsp_init_cuda() filled (tests/h264_dropin_cases.py).  Only in _ref. */
+ * picture in place through the loop-filter entries of `table` -- an H264DSPContext filled by anybody: NULL = ff_h264dsp_init(bit_depth, 1),
+ * the reference's C functions; otherwise e.g. the table ff_h264dsp_init_cuda() filled (tests/h264_dropin_cases.py).  At 9 / 10 bit the
+ * planes hold uint16 samples and ls / uvls count bytes; ref_h264_deblock_picture_with is the 8-bit call.  Only in _ref. */
+int ref_h264_deblock_picture_with_hbd(int bit_depth, const void *table, uint8_t *Y, uint8_t *Cb, uint8_t *Cr, int ls, int uvls,
+                                      int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
+                                      const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
+                                      const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
+                                      const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode)
+{
+    H264DSPContext c_table;
+    if (bit_depth < 8 || bit_depth > 10) return -1;
+    if (!table) { ff_h264dsp_init(&c_table, bit_depth, 1); table = &c_table; }
+    return run_driver(table, Y, Cb, Cr, ls, uvls, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1, slice_params, n_slices,
+                      chroma_qp_table, cabac, transform_8x8_mode, bit_depth, NULL);
+}
+
 int ref_h264_deblock_picture_with(const void *table, uint8_t *Y, uint8_t *Cb, uint8_t *Cr, int ls, int uvls,
                                   int mb_w, int mb_h, const uint32_t *mb_type, const int8_t *qscale, const uint8_t *nnz,
                                   const uint16_t *cbp, const uint16_t *slice_table, const int16_t *mv0, const int16_t *mv1,
                                   const int8_t *ref0, const int8_t *ref1, const int32_t *slice_params, int n_slices,
                                   const uint8_t *chroma_qp_table, int cabac, int transform_8x8_mode)
 {
-    H264DSPContext c_table;
-    if (!table) { ff_h264dsp_init(&c_table, 8, 1); table = &c_table; }
-    return run_driver(table, Y, Cb, Cr, ls, uvls, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1, slice_params, n_slices,
-                      chroma_qp_table, cabac, transform_8x8_mode, NULL);
+    return ref_h264_deblock_picture_with_hbd(8, table, Y, Cb, Cr, ls, uvls, mb_w, mb_h, mb_type, qscale, nnz, cbp, slice_table, mv0, mv1, ref0, ref1,
+                                             slice_params, n_slices, chroma_qp_table, cabac, transform_8x8_mode);
 }

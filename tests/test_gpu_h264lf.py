@@ -20,20 +20,31 @@ def _dev(a):
     return device.DevBuf.from_numpy(np.ascontiguousarray(a))
 
 
-def gpu_params(gpu, infos, field=0, chroma422=None):
-    """infos: list of per-picture dicts of equal geometry (stacked row-wise into one call)"""
-    from libav_b200 import device
+def device_info(infos, field=0, chroma422=None):
+    """(FFH264DeblockInfo, the device buffers it points at) for per-picture dicts of equal geometry, stacked row-wise; slice parameters and
+    chroma_qp_table are the first picture's"""
     d0 = infos[0]
     cat = lambda k: np.concatenate([d[k] for d in infos], axis=0)
     keep = {k: _dev(cat(k)) for k in ("mb_type", "qscale", "nnz", "cbp", "slice_table", "mv0", "mv1", "ref0", "ref1")}
     keep["sp"] = _dev(d0["slice_params"]); keep["cq"] = _dev(d0["chroma_qp_table"])
-    n = d0["mb_w"] * d0["mb_h"] * len(infos)
-    out = device.DevBuf(n * 104); out.fill(0xAB)
     info = tables.FFH264DeblockInfo(d0["mb_w"], d0["mb_h"], len(infos), keep["mb_type"].ptr, keep["qscale"].ptr, keep["nnz"].ptr,
                                     keep["cbp"].ptr, keep["slice_table"].ptr, (C.c_void_p * 2)(keep["mv0"].ptr, keep["mv1"].ptr),
                                     (C.c_void_p * 2)(keep["ref0"].ptr, keep["ref1"].ptr), keep["sp"].ptr, d0["n_slices"], keep["cq"].ptr,
                                     d0["cabac"], d0["t8x8"], field, chroma422)
-    gpu.check(gpu.lib.ff_h264_deblock_params_cuda(C.byref(info), out.ptr, None))
+    return info, keep
+
+
+def gpu_params(gpu, infos, field=0, chroma422=None, bits=None):
+    """infos: list of per-picture dicts of equal geometry (stacked row-wise into one call); bits: through ff_h264_deblock_params_hbd_cuda"""
+    from libav_b200 import device
+    d0 = infos[0]
+    info, keep = device_info(infos, field, chroma422)
+    n = d0["mb_w"] * d0["mb_h"] * len(infos)
+    out = device.DevBuf(n * 104); out.fill(0xAB)
+    if bits is None:
+        gpu.check(gpu.lib.ff_h264_deblock_params_cuda(C.byref(info), out.ptr, None))
+    else:
+        gpu.check(gpu.lib.ff_h264_deblock_params_hbd_cuda(bits, C.byref(info), out.ptr, None))
     device.sync()
     return out.download(np.uint8, (n, 104)), out
 

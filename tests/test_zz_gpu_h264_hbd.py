@@ -184,17 +184,20 @@ def test_intra_batch_hbd(gpu, checker, mb_w, mb_h, P, p_intra, bits):
 
 @pytest.mark.parametrize("bits", [9, 10])
 @pytest.mark.parametrize("mb_w,mb_h,P,p_intra", [(7, 5, 1, 0.3), (20, 12, 2, 0.25)])
-def test_flush_hbd_equals_the_chained_checker(gpu, checker, mb_w, mb_h, P, p_intra, bits):
+def test_flush_hbd_decides_at_the_streams_bit_depth(gpu, checker, mb_w, mb_h, P, p_intra, bits):
     """ff_h264_flush_pictures_cuda with bit_depth 9 / 10: MC -> weighted prediction -> DC transforms -> residual -> intra -> decisions -> loop filter in one
-    call, against the CPU checker's BIT_DEPTH > 8 functions chained in the same order on the same records"""
+    call, against the CPU checker's BIT_DEPTH > 8 functions chained in the same order on the same records; the checker decides at the stream's
+    bit depth"""
     import ctypes as C
     from libav_b200 import device, tables
     from oracle.loader import ptr
     from test_gpu_h264flush import picture_work
-    from test_oracle_h264lf_cpu import run as oracle_decisions
+    from test_oracle_h264lf_hbd_cpu import hbd_oracle, run as oracle_decisions
     sc = 1 << (bits - 8)
     refs = [hh.picture(mb_w, mb_h, bits, 0, seed=11), hh.picture(mb_w, mb_h, bits, 0, seed=12)]
     works = [picture_work(mb_w, mb_h, 100 * k + mb_w, p_intra) for k in range(P)]
+    for w in works:         # the side information a 9 / 10-bit decoder keeps: qscale_table, chroma_qp_table and qp_thresh in the QP' scale
+        w["info"] = synth.h264_deblock_info(mb_w, mb_h, seed=mb_w + 4, n_slices=3, bipred=True, t8x8=1, cabac=1, bit_depth=bits)
     pics = [hh.picture(mb_w, mb_h, bits, 0, seed=50 + k) for k in range(P)]
     ls, uvls = pics[0][0].strides[0], pics[0][1].strides[0]
     want, want_co = [], []
@@ -215,7 +218,7 @@ def test_flush_hbd_equals_the_chained_checker(gpu, checker, mb_w, mb_h, P, p_int
                     checker.h264_hbd_dc_dequant(bits, 1, hh.at(co, (m * 768 + 256 * (p + 1)) * 4), None, int(w["dc"]["chroma_qmul"][m, p]))
         hh.oracle_residual(checker, bits, 0, w["res"], co, w["nnzc"], wy, wcb, wcr)
         hh.oracle_intra(checker, bits, w["intra"], co, w["nnzc"], mb_w, mb_h, wy, wcb, wcr)
-        rec = oracle_decisions(checker, w["info"]).view(synth.DEBLOCK_DT).reshape(-1)
+        rec = oracle_decisions(hbd_oracle(checker), w["info"]).view(synth.DEBLOCK_DT).reshape(-1)
         hh.oracle_deblock(checker, bits, rec, mb_w, mb_h, wy, wcb, wcr)
         want.append((wy, wcb, wcr)); want_co.append(co)
     Y, CB, CR = (np.concatenate([p[i] for p in pics]) for i in range(3))
@@ -288,15 +291,27 @@ def test_flush_422_pictures(gpu, checker, mb_w, mb_h, P, p_intra, bits):
     """ff_h264_flush_pictures_cuda with chroma_format_idc 2 (8 and 10 bit), caller-filled deblocking records: MC -> weighted prediction -> DC transforms
     (2 x 4 chroma) -> residual -> intra macroblocks (8 x 16 chroma predictors) -> 4:2:2 loop filter in one call, against the CPU checker chained
     in the same order"""
+    flush_422(gpu, checker, mb_w, mb_h, P, p_intra, bits)
+
+
+def flush_422(gpu, checker, mb_w, mb_h, P, p_intra, bits, decide=False):
+    """decide: the flush derives the deblocking records from FFH264DeblockInfo (side information in the decoder's scale for `bits`, the
+    chroma422 array of the decisions); the checker decides at `bits` and both sets of records are compared as well as the pictures"""
     import ctypes as C
     from libav_b200 import device, tables
     from oracle.loader import ptr
+    from test_oracle_h264lf_hbd_cpu import hbd_oracle, run422
+    from test_gpu_h264lf import device_info
     sb = 1 if bits == 8 else 2
     cdt = np.int16 if bits == 8 else np.int32
     rng = np.random.default_rng(bits * 100 + mb_w)
     refs = [hh.smooth_picture422(mb_w, mb_h, bits, seed=11), hh.smooth_picture422(mb_w, mb_h, bits, seed=12)]
     n1 = mb_w * mb_h
     pics, mcs, ress, cos, nzs, dcs, wrecs, recs, exts, want, want_co, irecs = [], [], [], [], [], [], [], [], [], [], [], []
+    if decide:
+        infos = [synth.h264_deblock_info(mb_w, mb_h, seed=60 + k, n_slices=3, bipred=True, t8x8=1, bit_depth=bits) for k in range(P)]
+        for d_ in infos[1:]:                                                   # one set of slice headers / PPS per flush
+            d_["slice_params"], d_["chroma_qp_table"] = infos[0]["slice_params"], infos[0]["chroma_qp_table"]
     for k in range(P):
         y, cb, cr = hh.smooth_picture422(mb_w, mb_h, bits, seed=50 + k)
         ls, uvls = y.strides[0], cb.strides[0]
@@ -315,7 +330,11 @@ def test_flush_422_pictures(gpu, checker, mb_w, mb_h, P, p_intra, bits):
             if rng.random() < 0.4 and not intra[m]:
                 wr.append(((m // mb_w) * 16 * ls + (m % mb_w) * 16 * sb, 16, 16, int(rng.integers(0, 7)), 0, int(rng.integers(-20, 90)), 0, int(rng.integers(-20, 20)), 0))
         wr = np.array(wr, dtype=synth.WEIGHT_DT)
-        rec, ext = hh.deblock422_work(mb_w, mb_h, seed=3 + k, slices=2)
+        if decide:
+            rec, ext = run422(hbd_oracle(checker), infos[k])
+            rec, ext = rec.view(synth.DEBLOCK_DT).reshape(-1), ext.view(hh.CHROMA422_DT).reshape(-1)
+        else:
+            rec, ext = hh.deblock422_work(mb_w, mb_h, seed=3 + k, slices=2)
         wy, wcb, wcr, wco = y.copy(), cb.copy(), cr.copy(), co.copy()
         hh.oracle_mc(checker, bits, 1, mc, refs, wy, wcb, wcr)
         for r in wr:
@@ -360,10 +379,18 @@ def test_flush_422_pictures(gpu, checker, mb_w, mb_h, P, p_intra, bits):
     work.dc, work.luma_dc, work.residual = d["dc"].ptr, d["ldc"].ptr, d["res"].ptr
     if p_intra:
         work.intra = d["intra"].ptr
-    work.deblock_records, work.deblock_chroma422 = d["rec"].ptr, d["ext"].ptr
+    if decide:
+        d["rec"].fill(0xAB); d["ext"].fill(0xCD)
+        info, keep = device_info(infos, chroma422=d["ext"].ptr)
+        work.deblock_info, work.deblock_records = C.pointer(info), d["rec"].ptr
+    else:
+        work.deblock_records, work.deblock_chroma422 = d["rec"].ptr, d["ext"].ptr
     work.bit_depth, work.chroma_format_idc = bits, 2
     gpu.check(gpu.lib.ff_h264_flush_pictures_cuda(C.byref(work), None))
     device.sync()
+    if decide:
+        assert np.array_equal(d["rec"].download(np.uint8, (n, 104)), np.concatenate(recs).view(np.uint8).reshape(n, 104))
+        assert np.array_equal(d["ext"].download(np.uint8, (n, 52)), np.concatenate(exts).view(np.uint8).reshape(n, 52))
     gy, gcb, gcr = d["y"].download(Y.dtype, Y.shape), d["cb"].download(Y.dtype, CB.shape), d["cr"].download(Y.dtype, CR.shape)
     wy = np.concatenate([w[0] for w in want])
     assert np.array_equal(gy, wy), np.argwhere(gy != wy)[:5].tolist()
