@@ -22,6 +22,7 @@
 #include "libavcodec/h264pred.h"
 #include "libavcodec/hpeldsp.h"
 #include "libavcodec/pixblockdsp.h"
+#include "libavcodec/proresdsp.h"
 #include "libavcodec/qpeldsp.h"
 #include "libavcodec/fft.h"
 #include "libswscale/swscale.h"
@@ -43,6 +44,7 @@ void ff_pixblockdsp_init_cuda(PixblockDSPContext *c, unsigned high_bit_depth);
 void ff_qpeldsp_init_cuda(QpelDSPContext *c);
 void ff_h263dsp_init_cuda(H263DSPContext *c);
 void ff_mpegvideodsp_init_cuda(MpegVideoDSPContext *c);
+void ff_proresdsp_init_cuda(ProresDSPContext *dsp);
 void ff_fft_init_cuda(FFTContext *s);
 void ff_mdct_init_cuda(FFTContext *s);
 
@@ -90,6 +92,12 @@ void ff_pixblockdsp_init_cuda_hook(PixblockDSPContext *c, AVCodecContext *avctx,
 {
     (void)avctx;
     ff_pixblockdsp_init_cuda(c, high_bit_depth);
+}
+/* proresdsp.c:76-77: in place of ff_proresdsp_init_x86(dsp), before ff_init_scantable_permutation(); the CUDA slot wants
+ * FF_IDCT_PERM_NONE, the order of the C function, not the x86 code's transposed one */
+void ff_proresdsp_init_cuda_hook(ProresDSPContext *dsp)
+{
+    ff_proresdsp_init_cuda(dsp);
 }
 /* the remaining tables take exactly the arguments of their x86 hooks: ff_blockdsp_init_cuda(c), ff_me_cmp_init_cuda(c),
  * ff_h264dsp_init_cuda(c, bit_depth, chroma_format_idc), ff_h264qpel_init_cuda(c, bit_depth), ff_h264chroma_init_cuda(c, bit_depth),

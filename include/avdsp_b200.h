@@ -88,6 +88,49 @@ int ff_pixels_clamped_batch_cuda(int mode, const int16_t *blocks, uint8_t *frame
  * functions leave them.  Functional path for 10-bit content (thread per block), not tuned like the 8-bit kernel. */
 int ff_simple_idct10_batch_cuda(int mode, int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, size_t n, void *stream);
 
+/* ---- ProRes (libavcodec/proresdsp.c, proresdec.c) ---------------------------------------------------------------------------------------
+ * prores_idct_put_c over n blocks: block i is multiplied by the 64 int16 of qmats + 64 * qmat_idx[i] (matrix 0 for every block when
+ * qmat_idx is NULL; products wrap to int16), transformed by ff_prores_idct and written as av_clip(v + 512, 4, 1019) into the 8 x 8 16-bit
+ * samples at frame + dst_off[i] (bytes), rows `stride` bytes apart.  Each block is left as the C function leaves it: the column pass's
+ * int16 results.  Device pointers, on `stream`, without synchronising.  Blocks and qmats 16-byte aligned with a stride that is a multiple
+ * of 16 run the staged kernel, anything else a thread-per-block kernel.  Returns -1 for NULL pointers with n > 0 or an odd stride. */
+int ff_prores_idct_put_batch_cuda(int16_t *blocks, uint8_t *frame, const uint32_t *dst_off, ptrdiff_t stride, const int16_t *qmats,
+                                  const uint32_t *qmat_idx, size_t n, void *stream);
+
+/* One slice of a ProRes picture as decode_picture / decode_slice see it (device memory).  sf: the slice's scale factor after
+ * decode_slice's mapping (1..512); first_block: the slice's first coefficient block in FFProresPictureWork.blocks. */
+typedef struct FFProresSlice {
+    uint32_t first_block;
+    uint16_t sf;
+    uint16_t reserved;
+} FFProresSlice;
+/* One ProRes picture (a frame, or one field of an interlaced frame) whose slices were entropy-decoded but not transformed.  The
+ * coefficient buffer is in the decoder's order: per slice (raster order, as decode_picture numbers them), its luma blocks, then U, then V,
+ * each plane in decode_slice_plane's order (luma TL TR BL BR per macroblock; 4:2:2 chroma top, bottom; 4:4:4 chroma TL BL TR BR).
+ * The call derives each block's destination and scaled matrix (int16_t)(qmat[i] * sf) on the device.  Blocks inside the buffer that no
+ * slice covers are skipped. */
+typedef struct FFProresPictureWork {
+    uint8_t *data[3];            /* device: y, u, v as decode_slice computes them (a field's second picture starts one frame line down) */
+    int linesize[3];             /* bytes between the picture's lines (doubled for a field), even and > 0; at least the width of whole
+                                  * macroblocks (32 * mb_width bytes for luma and 4:4:4 chroma, 16 * mb_width for 4:2:2 chroma).  The call
+                                  * sees only this linesize: for a field it cannot tell a frame buffer narrower than whole macroblocks
+                                  * (whose two fields' rows then overlap) from a wide one, so the caller guarantees the frame linesize */
+    int mb_rows[3];              /* 16-line rows at linesize each plane buffer holds from data[p]: at least mb_height */
+    int mb_width, mb_height;     /* ctx->num_x_mbs, ctx->num_y_mbs (macroblock rows of this picture) */
+    int slice_width_factor;      /* 0..3 */
+    int chroma_format;           /* ctx->chroma_factor: 2 = 4:2:2, 3 = 4:4:4 */
+    uint8_t qmat_luma[64], qmat_chroma[64];     /* ctx->qmat_luma / qmat_chroma (FF_IDCT_PERM_NONE order) */
+    const FFProresSlice *slices; /* device, n_slices entries */
+    int n_slices;                /* must be the picture's slice count, mb_height * slices per row */
+    const int16_t *blocks;       /* device, n_blocks * 64 coefficients, left unchanged */
+    size_t n_blocks;
+} FFProresPictureWork;
+/* The flush point of a ProRes decoder: the inverse quantisation, IDCT and store of n pictures, on `stream`, without synchronising; nothing
+ * else is read or written (no alpha plane).  Every picture is checked before anything is launched; -1 for a NULL array, a chroma_format
+ * other than 2 / 3, slice_width_factor > 3, macroblock dimensions outside 1..8192, a NULL or odd plane pointer or linesize, planes too
+ * small for whole macroblocks (width or mb_rows), a slice count that does not cover the picture, or NULL slices / blocks. */
+int ff_prores_decode_pictures_cuda(const FFProresPictureWork *pictures /* host array */, int n, void *stream);
+
 /* ff_xvid_idct / xvid_idct_put / xvid_idct_add (libavcodec/xvididct.c:272-331) over n blocks -- the IDCT ff_xvid_idct_init() installs for
  * MPEG-4 streams written by Xvid and for idct_algo FF_IDCT_XVID.  Arguments, addressing, mode 0 / 1 / 2 and `clear` exactly as
  * ff_simple_idct_batch_cuda; mode 2 leaves the transform result in the blocks.  Blocks at any 2-byte alignment and destinations at any
@@ -762,6 +805,9 @@ void ff_idctdsp_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sam
  * FF_IDCT_PERM_NONE and an identity idct_permutation when bits_per_raw_sample <= 8 and idct_algo is FF_IDCT_AUTO or FF_IDCT_XVID
  * (AVB_FF_IDCT_XVID); otherwise `c` is untouched.  ff_idctdsp_init_cuda leaves FF_IDCT_XVID alone, like the reference's ff_idctdsp_init. */
 void ff_xvid_idct_init_cuda(IDCTDSPContext *c, int idct_algo, int bits_per_raw_sample);
+/* libavcodec/proresdsp.c:70-80 without the x86 part: idct_put = the slot of prores_idct_put_c (a batch of one of
+ * ff_prores_idct_put_batch_cuda with host pointers), idct_permutation_type = FF_IDCT_PERM_NONE and the identity permutation. */
+void ff_proresdsp_init_cuda(ProresDSPContext *dsp);
 void ff_blockdsp_init_cuda(BlockDSPContext *c);   /* libavcodec/blockdsp.c:60-74 */
 /* libavcodec/fdctdsp.c:27-50 (same shape as ff_fdctdsp_init_x86): dct_algo FF_DCT_AUTO / FF_DCT_INT -> islow,
  * FF_DCT_FASTINT -> ifast, FF_DCT_FAAN -> ff_faandct / ff_faandct248; bits_per_raw_sample 10 -> jpeg_fdct_islow_10 / fdct248_islow_10

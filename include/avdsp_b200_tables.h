@@ -40,6 +40,13 @@ typedef struct IDCTDSPContext {
 #define AVB_FF_IDCT_XVID   14
 #define AVB_FF_IDCT_FAAN   20
 
+/* ---- libavcodec/proresdsp.h:31-35 ---- */
+typedef struct ProresDSPContext {
+    int idct_permutation_type;
+    uint8_t idct_permutation[64];
+    void (*idct_put)(uint16_t *out, ptrdiff_t linesize, int16_t *block, const int16_t *qmat);
+} ProresDSPContext;
+
 /* ---- libavcodec/fdctdsp.h:26-29 ---- */
 typedef struct FDCTDSPContext {
     void (*fdct)(int16_t *block);

@@ -58,6 +58,8 @@ PROTOTYPES = {
     "avb200_event_elapsed_ms": (C.c_float, [vp, vp]),
     "ff_simple_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_simple_idct10_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, vp]),
+    "ff_prores_idct_put_batch_cuda": (i32, [vp, vp, vp, pd, vp, vp, sz, vp]),
+    "ff_prores_decode_pictures_cuda": (i32, [vp, i32, vp]),
     "ff_xvid_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_faanidct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_pixels_clamped_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, vp]),
@@ -117,6 +119,7 @@ PROTOTYPES = {
     "sws_debug_slot_view_cuda": (i32, [i32, i32, i32, i32, i32, i32, i32, vp]),
     "ff_idctdsp_init_cuda": (None, [vp, i32, i32, C.c_uint]),
     "ff_xvid_idct_init_cuda": (None, [vp, i32, i32]),
+    "ff_proresdsp_init_cuda": (None, [vp]),
     "ff_blockdsp_init_cuda": (None, [vp]),
     "ff_fdctdsp_init_cuda": (None, [vp, i32, i32, C.c_uint]),
     "ff_me_cmp_init_cuda": (None, [vp]),

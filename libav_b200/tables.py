@@ -17,6 +17,22 @@ class IDCTDSPContext(C.Structure):          # libavcodec/idctdsp.h:53-98
                 ("idct_permutation", C.c_uint8 * 64), ("perm_type", C.c_int)]
 
 
+class ProresDSPContext(C.Structure):        # libavcodec/proresdsp.h:31-35
+    _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
+                ("idct_put", C.CFUNCTYPE(None, C.POINTER(C.c_uint16), pd, i16p, i16p))]
+
+
+class FFProresSlice(C.Structure):           # include/avdsp_b200.h
+    _fields_ = [("first_block", C.c_uint32), ("sf", C.c_uint16), ("reserved", C.c_uint16)]
+
+
+class FFProresPictureWork(C.Structure):     # include/avdsp_b200.h
+    _fields_ = [("data", C.c_void_p * 3), ("linesize", C.c_int * 3), ("mb_rows", C.c_int * 3), ("mb_width", C.c_int),
+                ("mb_height", C.c_int), ("slice_width_factor", C.c_int), ("chroma_format", C.c_int),
+                ("qmat_luma", C.c_uint8 * 64), ("qmat_chroma", C.c_uint8 * 64), ("slices", C.c_void_p), ("n_slices", C.c_int),
+                ("blocks", C.c_void_p), ("n_blocks", C.c_size_t)]
+
+
 class FDCTDSPContext(C.Structure):          # libavcodec/fdctdsp.h:26-29
     _fields_ = [("fdct", _idct), ("fdct248", _idct)]
 
