@@ -131,6 +131,37 @@ typedef struct FFProresPictureWork {
  * small for whole macroblocks (width or mb_rows), a slice count that does not cover the picture, or NULL slices / blocks. */
 int ff_prores_decode_pictures_cuda(const FFProresPictureWork *pictures /* host array */, int n, void *stream);
 
+/* ---- ProRes encoder (libavcodec/proresenc.c) --------------------------------------------------------------------------------------------
+ * One frame for ff_prores_encode_frames_cuda: the source planes and the encoder's options, as encode_init / encode_frame take them. */
+typedef struct FFProresEncodeWork {
+    const uint8_t *data[4];      /* device: y, u, v (and alpha for yuva444p10) planes of 16-bit samples in 0..1023, even addresses */
+    int linesize[4];             /* bytes between lines, even, at least the plane's width in bytes (4:2:2 chroma: (width + 1) / 2 samples) */
+    int width, height;           /* 1..65535; interlaced heights 1 and 32k + 1 are refused (a field's last macroblock row has no lines) */
+    int pix_fmt;                 /* 0 yuv422p10, 1 yuv444p10, 2 yuva444p10 */
+    int interlaced;              /* 0 progressive, 1 top field first, 2 bottom field first (AV_CODEC_FLAG_INTERLACED_DCT + top_field_first) */
+    int profile;                 /* 0..4: proxy, LT, standard, HQ, 4444 (the encoder's "profile" option) */
+    int mbs_per_slice;           /* 1, 2, 4, 8 */
+    int bits_per_mb;             /* 0 = from the profile's table for the frame size, else 128..8192 (ignored under force_quant) */
+    int quant_sel;               /* -1 = the profile's matrix, 0..4 (the "quant_mat" option; 4 = default, not written to the header) */
+    int alpha_bits;              /* 0, 8, 16; only read for yuva444p10 */
+    int force_quant;             /* 0 = rate control, 1..64 = one quantiser for every slice (global_quality / FF_QP2LAMBDA) */
+    char vendor[4];              /* four non-zero bytes */
+    uint8_t color_primaries, color_trc, colorspace;
+    uint8_t *out;                /* device packet buffer */
+    size_t out_capacity;
+    int32_t *out_size;           /* device, 4-byte aligned: the packet's size, or -(size needed) with out untouched when it does not fit */
+} FFProresEncodeWork;
+/* Bytes of device workspace ff_prores_encode_frames_cuda needs for these frames (host only, nothing launched); 0 for a refused batch. */
+size_t ff_prores_encode_workspace_cuda(const FFProresEncodeWork *frames /* host array */, int n);
+/* encode_frame for n frames on `stream`, without synchronising: each packet is the reference encoder's for the same frame and options, byte
+ * for byte, with find_quant_thread's rate control (or force_quant) and every slice coded on the device.  Every frame is checked before
+ * anything is launched; -1 with a message for what encode_init refuses (pix_fmt, interlaced, profile or quant_sel out of range,
+ * mbs_per_slice not 1 / 2 / 4 / 8, alpha_bits not 0 / 8 / 16, bits_per_mb in 1..127 without force_quant or above 8192, force_quant outside
+ * 0..64, a vendor ID with a zero byte), NULL or odd planes, odd or narrow linesizes, sizes the headers cannot hold (width or height outside
+ * 1..65535, more than 65535 slices per picture), interlaced heights 1 and 32k + 1, a NULL out / out_size, and a workspace smaller than
+ * ff_prores_encode_workspace_cuda returns. */
+int ff_prores_encode_frames_cuda(const FFProresEncodeWork *frames /* host array */, int n, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ff_xvid_idct / xvid_idct_put / xvid_idct_add (libavcodec/xvididct.c:272-331) over n blocks -- the IDCT ff_xvid_idct_init() installs for
  * MPEG-4 streams written by Xvid and for idct_algo FF_IDCT_XVID.  Arguments, addressing, mode 0 / 1 / 2 and `clear` exactly as
  * ff_simple_idct_batch_cuda; mode 2 leaves the transform result in the blocks.  Blocks at any 2-byte alignment and destinations at any

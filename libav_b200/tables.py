@@ -33,6 +33,14 @@ class FFProresPictureWork(C.Structure):     # include/avdsp_b200.h
                 ("blocks", C.c_void_p), ("n_blocks", C.c_size_t)]
 
 
+class FFProresEncodeWork(C.Structure):      # include/avdsp_b200.h
+    _fields_ = [("data", C.c_void_p * 4), ("linesize", C.c_int * 4), ("width", C.c_int), ("height", C.c_int), ("pix_fmt", C.c_int),
+                ("interlaced", C.c_int), ("profile", C.c_int), ("mbs_per_slice", C.c_int), ("bits_per_mb", C.c_int),
+                ("quant_sel", C.c_int), ("alpha_bits", C.c_int), ("force_quant", C.c_int), ("vendor", C.c_char * 4),
+                ("color_primaries", C.c_uint8), ("color_trc", C.c_uint8), ("colorspace", C.c_uint8), ("out", C.c_void_p),
+                ("out_capacity", C.c_size_t), ("out_size", C.c_void_p)]
+
+
 class FDCTDSPContext(C.Structure):          # libavcodec/fdctdsp.h:26-29
     _fields_ = [("fdct", _idct), ("fdct248", _idct)]
 
