@@ -162,6 +162,61 @@ size_t ff_prores_encode_workspace_cuda(const FFProresEncodeWork *frames /* host 
  * ff_prores_encode_workspace_cuda returns. */
 int ff_prores_encode_frames_cuda(const FFProresEncodeWork *frames /* host array */, int n, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- VC-3 / DNxHD encoder (libavcodec/dnxhdenc.c) -----------------------------------------------------------------------------------------
+ * CIDEntry (libavcodec/dnxhddata.h:28-42), field for field: the encoder's ctx->cid_table.  The library builds its device VLC, run and
+ * weight tables from the entry, caches them by the entry's host address and rebuilds them when a checksum of the arrays changes. */
+typedef struct FFDnxhdCidEntry {
+    int cid;
+    unsigned int width, height;
+    int interlaced;
+    unsigned int frame_size;
+    unsigned int coding_unit_size;
+    int index_bits;
+    int bit_depth;
+    const uint8_t *luma_weight, *chroma_weight;
+    const uint8_t *dc_codes, *dc_bits;
+    const uint16_t *ac_codes;
+    const uint8_t *ac_bits, *ac_level;
+    const uint8_t *ac_run_flag, *ac_index_flag;
+    const uint16_t *run_codes;
+    const uint8_t *run_bits, *run;
+    int bit_rates[5];
+} FFDnxhdCidEntry;
+/* The rate-control state that DNXHDEncContext carries from field to field and frame to frame; a new encoder starts at { 1, 2 << 10 }
+ * (dnxhd_init_rc).  The fast rate control needs qscale in 1..qmax - 1, where the encoder leaves it; a frame that finds it elsewhere fails
+ * with EINVAL.  After a failure the state is what the reference leaves: the last qscale find_qscale tried, lambda untouched by RD. */
+typedef struct FFDnxhdRcState { uint32_t qscale, lambda; } FFDnxhdRcState;
+/* One frame for ff_dnxhd_encode_frames_cuda, as dnxhd_encode_picture takes it. */
+typedef struct FFDnxhdEncodeWork {
+    const uint8_t *data[3];      /* device planes: yuv422p (8-bit samples) or yuv422p10 (16-bit samples in 0..1023, even addresses).  For
+                                  * 1080-line 10-bit CIDs the luma plane must have 1088 readable lines: the variance pass of the fast rate
+                                  * control reads all 16 lines of the last macroblock row, as dnxhd_mb_var_thread does, and those 8 lines
+                                  * change the packet */
+    int linesize[3];             /* bytes between lines, positive; even at 10 bit; at least the plane's width in bytes */
+    const FFDnxhdCidEntry *cid_table;  /* host: the entry the encoder chose (ff_dnxhd_cid_table[i]); size, interlacing, bit depth */
+    int interlaced;              /* 0 progressive, 1 top field first, 2 bottom field first (cur_field of dnxhd_load_picture); must match
+                                  * cid_table->interlaced */
+    int dct_algo;                /* 8 bit only: FF_DCT_FASTINT (1) ifast, FF_DCT_FAAN (6) FAAN, anything else islow */
+    int mb_decision;             /* FF_MB_DECISION_RD (2): dnxhd_encode_rdo; anything else: dnxhd_encode_fast */
+    int qmax;                    /* 2..69 */
+    int nitris_compat;           /* 0 or 1 (min_padding 1600) */
+    FFDnxhdRcState *state;       /* device; frames sharing a pointer are encoded in array order, as one context encodes them */
+    uint8_t *out;                /* device, 4-byte aligned: cid_table->frame_size bytes are written, never more */
+    size_t out_capacity;         /* at least cid_table->frame_size */
+    int32_t *out_info;           /* device: [0] the packet size (frame_size) or AVERROR(EINVAL) when rate control cannot fit the picture
+                                  * (the packet bytes are then unspecified), [1] qscale * FF_QP2LAMBDA, the quality side data (with
+                                  * FF_MB_DECISION_RD qscale is qmax - 1, where dnxhd_encode_rdo's table loop leaves ctx->qscale) */
+} FFDnxhdEncodeWork;
+/* Bytes of device workspace ff_dnxhd_encode_frames_cuda needs for these frames (host only, nothing launched); 0 for a refused batch. */
+size_t ff_dnxhd_encode_workspace_cuda(const FFDnxhdEncodeWork *frames /* host array */, int n);
+/* dnxhd_encode_picture for n frames on `stream`, without synchronising: each packet is the reference encoder's for the same frame, options
+ * and state, byte for byte, and each state is left as the encoder leaves its context, after a rate-control failure too.  Every frame is
+ * checked before anything is launched; -1 with a message for NULL or odd planes and linesizes, linesizes narrower than the plane, a CID
+ * entry with a bit depth other than 8 / 10 or one dnxhd_init_vlc would reject (a level without a code, a run of 0 or past 62, a run listed
+ * twice), interlacing that does not match the entry, qmax outside 2..69, nitris_compat not 0 / 1, out_capacity below frame_size, a NULL or
+ * misaligned out, a NULL state or out_info, and a workspace smaller than ff_dnxhd_encode_workspace_cuda returns. */
+int ff_dnxhd_encode_frames_cuda(const FFDnxhdEncodeWork *frames /* host array */, int n, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ff_xvid_idct / xvid_idct_put / xvid_idct_add (libavcodec/xvididct.c:272-331) over n blocks -- the IDCT ff_xvid_idct_init() installs for
  * MPEG-4 streams written by Xvid and for idct_algo FF_IDCT_XVID.  Arguments, addressing, mode 0 / 1 / 2 and `clear` exactly as
  * ff_simple_idct_batch_cuda; mode 2 leaves the transform result in the blocks.  Blocks at any 2-byte alignment and destinations at any

@@ -41,6 +41,25 @@ class FFProresEncodeWork(C.Structure):      # include/avdsp_b200.h
                 ("out_capacity", C.c_size_t), ("out_size", C.c_void_p)]
 
 
+class FFDnxhdCidEntry(C.Structure):         # include/avdsp_b200.h (CIDEntry, libavcodec/dnxhddata.h:28-42)
+    _fields_ = [("cid", C.c_int), ("width", C.c_uint), ("height", C.c_uint), ("interlaced", C.c_int), ("frame_size", C.c_uint),
+                ("coding_unit_size", C.c_uint), ("index_bits", C.c_int), ("bit_depth", C.c_int),
+                ("luma_weight", C.c_void_p), ("chroma_weight", C.c_void_p), ("dc_codes", C.c_void_p), ("dc_bits", C.c_void_p),
+                ("ac_codes", C.c_void_p), ("ac_bits", C.c_void_p), ("ac_level", C.c_void_p), ("ac_run_flag", C.c_void_p),
+                ("ac_index_flag", C.c_void_p), ("run_codes", C.c_void_p), ("run_bits", C.c_void_p), ("run", C.c_void_p),
+                ("bit_rates", C.c_int * 5)]
+
+
+class FFDnxhdRcState(C.Structure):          # include/avdsp_b200.h
+    _fields_ = [("qscale", C.c_uint32), ("lambda_", C.c_uint32)]
+
+
+class FFDnxhdEncodeWork(C.Structure):       # include/avdsp_b200.h
+    _fields_ = [("data", C.c_void_p * 3), ("linesize", C.c_int * 3), ("cid_table", C.c_void_p), ("interlaced", C.c_int),
+                ("dct_algo", C.c_int), ("mb_decision", C.c_int), ("qmax", C.c_int), ("nitris_compat", C.c_int), ("state", C.c_void_p),
+                ("out", C.c_void_p), ("out_capacity", C.c_size_t), ("out_info", C.c_void_p)]
+
+
 class FDCTDSPContext(C.Structure):          # libavcodec/fdctdsp.h:26-29
     _fields_ = [("fdct", _idct), ("fdct248", _idct)]
 
