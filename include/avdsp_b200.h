@@ -841,6 +841,7 @@ int ff_mdct_batch_cuda(int op, int nbits, double scale, float *out, const float 
  *                          0 on bad arguments.
  *   sws_scale_frames_cuda  DEVICE pointers, asynchronous on `stream`: nframes frames whose planes lie
  *                          *_frame_stride[] bytes apart (NULL = a single frame); returns lines written or -1.
+ *                          Calls on one context must be ordered: one stream, or streams the caller synchronises.
  *                          For odd dstW the reference writes whole pixel pairs (libswscale/output.c:947); that
  *                          extra pixel is written only when dst_stride >= 3 * (dstW + 1). */
 #define AVB_PIX_FMT_YUV420P 0

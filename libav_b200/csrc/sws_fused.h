@@ -38,9 +38,10 @@ __device__ __forceinline__ int sat255(int v) { return __vimin_s32_relu(v, 255); 
 
 #ifndef AVB_HOSTSIM
 // 0 launched, -1 error (sticky message set), 1 not applicable (pitches / pointers the tensor maps cannot describe): the caller runs
-// the LDG kernel instead.  `taps` is the device copy of SwsPairTapsT[dstH / 2].
+// the LDG kernel instead.  `taps` is the device copy of SwsPairTapsT[dstH / 2].  `tickets` is the kernel's tile counter: one int,
+// zero before the first launch, which every launch leaves at zero; launches that share it must be ordered on one stream.
 int sws_fused_tma_launch(const RgbConstants &k, int bgr, int dstW, int dstH, int chrSrcW, int chrSrcH, const FusedArgs &a,
-                         const SwsPairTapsT *taps, int nframes, cudaStream_t st);
+                         const SwsPairTapsT *taps, int *tickets, int nframes, cudaStream_t st);
 #endif
 
 }  // namespace avb

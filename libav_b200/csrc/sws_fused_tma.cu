@@ -6,8 +6,8 @@
 //   * a warp owns a 256 x 8 pixel tile (four row pairs).  Its luma rows (8 x 256 B) and the eight chroma lines of each plane that the
 //     tile's vertical windows touch (8 x 128 B each) arrive by three cp.async.bulk.tensor (TMA, 3-D maps x / line / frame, zero fill
 //     outside the plane) into one of the warp's own three stages and are awaited on that stage's mbarrier: no CTA-wide barrier exists
-//     after start-up, the next two tiles are always in flight.  Warps are persistent and stride over the tiles of all frames of the
-//     batch.
+//     after start-up, the next two tiles are always in flight.  Warps are persistent: each takes its first FT_FIXED tiles by a fixed
+//     stride over the tiles of all frames of the batch and the rest from a tile counter, so that all warps finish together.
 //   * a thread owns 16 pixels x 4 rows (row pairs `half` and `half + 2` of the tile).  The seven chroma lines they need are
 //     byte-transposed once (window 0-3), the windows of the next rows are one PRMT away (drop the oldest line, append the next); the
 //     4-tap FIR is two IDP.2A on int16 taps.
@@ -32,6 +32,11 @@ namespace {
 
 constexpr int FT_STAGE = 4096;                  // Y 8 rows x 256 B | U 8 lines x 128 B | V 8 lines x 128 B
 constexpr int FT_STAGES = 3;                    // tile stages per warp
+// Tiles per warp by the fixed stride before the tile counter's.  The first ticket is drawn on the way to the last fixed tile: with
+// only the pipeline's first tiles fixed, all warps draw it at once, in one burst on one address, at the start of the launch; 6, 8
+// and 12 measured alike and about 1 % faster per step than 3 (profiles/README.md).
+constexpr int FT_FIXED = 8;
+static_assert(FT_FIXED >= 2, "the first ticket is drawn on the way to the last fixed tile");
 constexpr int FT_OUT = 4 * 768;                 // output staging: four 768-byte rows (half a tile) per bulk tensor store
 constexpr int FT_LUTC = 8;                      // lane copies of each term table entry
 constexpr int FT_LUT_BYTES = 2 * 256 * FT_LUTC * 8;     // table by V {tr, tgv}, table by U {tb, tgu}: 256 entries x FT_LUTC copies x 8 B
@@ -98,7 +103,7 @@ __device__ __forceinline__ void row16(const uint32_t (&TU)[8], const uint32_t (&
 
 template <bool BGR>
 __global__ void __launch_bounds__(FT_BOUND_THREADS, 1)
-sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const SwsPairTapsT *__restrict__ taps,
+sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const SwsPairTapsT *__restrict__ taps, int *tickets,
                            const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmV,
                            const __grid_constant__ CUtensorMap tmD)
 {
@@ -132,7 +137,7 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
     const int cg = lane & 15, half = lane >> 4;
     const unsigned lutV_s = smem_s + (cg % FT_LUTC) * 8, lutU_s = smem_s + 256 * FT_LUTC * 8 + (cg % FT_LUTC) * 8;
 
-    int item = blockIdx.x * nwarps + warp;
+    const int item = blockIdx.x * nwarps + warp;
     if (item >= a.nitems) return;
     const int wstride = gridDim.x * nwarps;
     const uint64_t evict_first = l2_policy_evict_first();
@@ -143,6 +148,14 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
         if (ty >= a.nTy) { ty -= a.nTy; f++; }
     };
     auto tile_words = [&](int ty) { return __ldg(reinterpret_cast<const int2 *>(&taps[a.rp0 + 4 * ty].base)); };   // (base, interior)
+    // A warp's first FT_FIXED tiles are fixed (item + s * wstride); the rest are handed out by the ticket counter in order (tx, then
+    // tile row, then frame), so that a warp that runs faster takes more tiles and the warps end together.  Lane 0 draws each ticket
+    // one tile before the warp reads it.  Every warp draws until it gets a ticket past the last tile, once; the warp that draws the
+    // last of those wstride failing tickets puts the counter back to 0 for the next launch on the stream, which reads it only after
+    // its own griddepcontrol.wait.
+    const long long nfixed = (long long)FT_FIXED * wstride;
+    const bool dyn = a.nitems > nfixed;
+    const int nlast = dyn ? (int)(a.nitems - nfixed) + wstride - 1 : 0;
     auto issue = [&](int tx, int ty, int f, int base, unsigned st) {
         if (lane == 0) {
             const unsigned mb = mbar_s + 8 * st, dst = stage_s + st * FT_STAGE;
@@ -153,30 +166,50 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
             tma_load_3d(dst + 3072, &tmV, tx * 128, base, f, mb);
         }
     };
-    // The tile being computed (c) and the tile issued next (n, FT_STAGES - 1 strides ahead) are tracked by coordinates; the table words
-    // of n are fetched a whole tile before its loads are issued, those of the tiles in flight are kept in q (oldest first).
-    int ctx = item % a.tilesX, cty, cf;
-    { const int t2 = item / a.tilesX; cty = t2 % a.nTy; cf = t2 / a.nTy; }
-    int ntx = ctx, nty = cty, nf = cf;
+    // The tile issued next (n, FT_STAGES - 1 tiles ahead) is tracked by item and coordinates; the table words of n are fetched a whole
+    // tile before its loads are issued; the items and words of the tiles in flight are kept in qi and q (oldest first).
+    int ntx = item % a.tilesX, nty, nf;
+    { const int t2 = item / a.tilesX; nty = t2 % a.nTy; nf = t2 / a.nTy; }
     long long nitem = item;
+    int ticket = 0;                                   // lane 0: the ticket drawn ahead
+    auto next = [&]() {
+        if (!dyn || nitem < nfixed - 2 * wstride) { nitem += wstride; advance(ntx, nty, nf); }
+        else if (nitem < nfixed - wstride) {          // on to the last fixed tile: draw the first ticket
+            nitem += wstride; advance(ntx, nty, nf);
+            if (lane == 0) ticket = atomicAdd(tickets, 1);
+        } else if (nitem < a.nitems) {
+            const int t = __shfl_sync(0xffffffffu, ticket, 0);
+            nitem = nfixed + t;
+            if (nitem < a.nitems) {
+                ntx = (int)(nitem % a.tilesX);
+                const int t2 = (int)(nitem / a.tilesX); nty = t2 % a.nTy; nf = t2 / a.nTy;
+                if (lane == 0) ticket = atomicAdd(tickets, 1);
+            } else if (t == nlast && lane == 0) {
+                atomicExch(tickets, 0);
+            }
+        }
+    };
     int2 q[FT_STAGES - 1];
+    int qi[FT_STAGES - 1];
 #pragma unroll
     for (int s = 0; s < FT_STAGES - 1; s++) {
+        qi[s] = (int)min(nitem, (long long)a.nitems);
         q[s] = nitem < a.nitems ? tile_words(nty) : make_int2(0, 0);
         if (nitem < a.nitems) issue(ntx, nty, nf, q[s].x, s);
-        advance(ntx, nty, nf); nitem += wstride;
+        next();
     }
     int2 nw = nitem < a.nitems ? tile_words(nty) : make_int2(0, 0);
 
     unsigned st = 0, phase = 0;
-    for (; item < a.nitems; item += wstride) {
+    while (qi[0] < a.nitems) {
         const int2 cw = q[0];
-        // the stage computed last (st - 1) is free again: the tile FT_STAGES - 1 strides ahead starts travelling before this one is touched
+        const int ctx = qi[0] % a.tilesX, ct2 = qi[0] / a.tilesX, cty = ct2 % a.nTy, cf = ct2 / a.nTy;
+        // the stage computed last (st - 1) is free again: the tile FT_STAGES - 1 tiles ahead starts travelling before this one is touched
         if (nitem < a.nitems) issue(ntx, nty, nf, nw.x, st == 0 ? FT_STAGES - 1 : st - 1);
 #pragma unroll
-        for (int s = 0; s < FT_STAGES - 2; s++) q[s] = q[s + 1];
-        q[FT_STAGES - 2] = nw;
-        advance(ntx, nty, nf); nitem += wstride;
+        for (int s = 0; s < FT_STAGES - 2; s++) { q[s] = q[s + 1]; qi[s] = qi[s + 1]; }
+        q[FT_STAGES - 2] = nw; qi[FT_STAGES - 2] = (int)min(nitem, (long long)a.nitems);
+        next();
         nw = nitem < a.nitems ? tile_words(nty) : make_int2(0, 0);
 
         const int rpT = a.rp0 + 4 * cty;
@@ -252,7 +285,6 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
             }
             __syncwarp();
         }
-        advance(ctx, cty, cf);
         if (++st == FT_STAGES) { st = 0; phase ^= 1u; }
     }
     if (lane == 0) bulk_wait<0>();
@@ -261,7 +293,7 @@ sws_fused_rgb24_tma_kernel(const RgbConstants k, const FusedTmaArgs a, const Sws
 }  // namespace
 
 int sws_fused_tma_launch(const RgbConstants &k, int bgr, int dstW, int dstH, int chrSrcW, int chrSrcH, const FusedArgs &a,
-                         const SwsPairTapsT *taps, int nframes, cudaStream_t st)
+                         const SwsPairTapsT *taps, int *tickets, int nframes, cudaStream_t st)
 {
     const int pairs = dstH / 2;
     const int rp0 = a.rp0, rp1 = a.rp1 < pairs ? a.rp1 : pairs;
@@ -332,7 +364,7 @@ int sws_fused_tma_launch(const RgbConstants &k, int bgr, int dstW, int dstH, int
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    if (cudaLaunchKernelEx(&cfg, kern, k, fa, taps, tmY, tmU, tmV, tmD) != cudaSuccess) { set_error("sws_scale:fused tma", cudaGetLastError()); return -1; }
+    if (cudaLaunchKernelEx(&cfg, kern, k, fa, taps, tickets, tmY, tmU, tmV, tmD) != cudaSuccess) { set_error("sws_scale:fused tma", cudaGetLastError()); return -1; }
     return check_launch("sws_scale:fused tma");
 }
 

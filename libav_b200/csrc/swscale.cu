@@ -1395,6 +1395,9 @@ struct SwsCudaContext {
     void *d_pair_taps = nullptr; // SwsPairTaps[dstH / 2] for the dp4a fused kernel (fast_ok only)
     void *d_pair_taps_t = nullptr; // SwsPairTapsT[dstH / 2] for the TMA fused kernel (tma_ok only)
     bool tma_ok = false;        // every four-pair tile of the TMA kernel reaches at most eight chroma lines
+    // the TMA kernel's tile counters (tma_ok only): one for launches on the caller's stream, one for each of `streams`.  Launches that
+    // share a counter must be ordered, so the device-pointer calls of a context go to one stream, or to streams the caller orders.
+    int *d_tickets = nullptr;
     SwsDev dev;
     int16_t *d_lum = nullptr, *d_chrU = nullptr, *d_chrV = nullptr;   // general path line planes
     int lumStridePx = 0, chrStridePx = 0;
@@ -1420,7 +1423,7 @@ static void destroy(SwsCudaContext *c)
 {
     if (!c) return;
     if (c->streams_ok) for (int i = 0; i < 3; i++) cudaStreamDestroy(c->streams[i]);
-    cudaFree(c->d_pal); cudaFree(c->d_tables); cudaFree(c->d_pair_taps); cudaFree(c->d_pair_taps_t); cudaFree(c->d_nv); cudaFree(c->d_rgb); cudaFree(c->d_tile_win); cudaFree(c->d_lum); cudaFree(c->d_chrU); cudaFree(c->d_chrV); cudaFree(c->d_src); cudaFree(c->d_dst); cudaFree(c->d_gray[0]); cudaFree(c->d_gray[1]);
+    cudaFree(c->d_pal); cudaFree(c->d_tables); cudaFree(c->d_pair_taps); cudaFree(c->d_pair_taps_t); cudaFree(c->d_tickets); cudaFree(c->d_nv); cudaFree(c->d_rgb); cudaFree(c->d_tile_win); cudaFree(c->d_lum); cudaFree(c->d_chrU); cudaFree(c->d_chrV); cudaFree(c->d_src); cudaFree(c->d_dst); cudaFree(c->d_gray[0]); cudaFree(c->d_gray[1]);
     delete c;
 }
 
@@ -1734,7 +1737,10 @@ static SwsCudaContext *make_context(int srcW, int srcH, int srcFormat, int dstW,
             for (int rp = t0; rp < t1; rp++) { pt[rp].base = lo; pt[rp].interior = interior; }
         }
         if (ok && pairs > 0) {
-            if (upload(&c->d_pair_taps_t, pt.data(), pt.size() * sizeof(SwsPairTapsT))) { destroy(c); return nullptr; }
+            static const int zero4[4] = { 0, 0, 0, 0 };
+            if (upload(&c->d_pair_taps_t, pt.data(), pt.size() * sizeof(SwsPairTapsT)) || upload((void **)&c->d_tickets, zero4, sizeof(zero4))) {
+                destroy(c); return nullptr;
+            }
             c->tma_ok = true;
         }
     }
@@ -1851,7 +1857,10 @@ static int launch_fused_fast(SwsCudaContext *c, const FusedArgs &a, int nframes,
     const SwsDev &p = c->dev;
 #ifndef AVB_HOSTSIM
     if (c->tma_ok) {
-        const int r = sws_fused_tma_launch(p.k, p.bgr, p.dstW, p.dstH, p.chrSrcW, p.chrSrcH, a, (const SwsPairTapsT *)c->d_pair_taps_t, nframes, st);
+        int slot = 0;               // the counter of the stream (SwsCudaContext::d_tickets)
+        for (int i = 0; i < 3; i++) if (c->streams_ok && st == c->streams[i]) slot = 1 + i;
+        const int r = sws_fused_tma_launch(p.k, p.bgr, p.dstW, p.dstH, p.chrSrcW, p.chrSrcH, a, (const SwsPairTapsT *)c->d_pair_taps_t,
+                                           c->d_tickets + slot, nframes, st);
         if (r <= 0) return r;
     }
 #endif
