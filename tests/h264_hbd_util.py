@@ -80,9 +80,17 @@ def oracle_residual(o, bits, c422, rec, coeffs, nnzc, y, cb, cr):
             idct_mb(4 if c422 else 3, None, d2, blk, uvls, nz)
 
 
-def oracle_mc(o, bits, c422, rec, refs, y, cb, cr, pad=48):
-    """refs: list of (y, cb, cr) uint16 planes; emulated_edge_mc = edge-replicated padding of the reference planes"""
-    pr = [tuple(np.pad(p, pad, mode="edge") for p in r) for r in refs]
+def oracle_mc(o, bits, c422, rec, refs, y, cb, cr, pw=None, ph=None):
+    """refs: list of (y, cb, cr) planes (uint16 above 8 bit); emulated_edge_mc = the reference planes cropped to pw x ph (default: the
+    destination's size) and edge-replicated as far as the farthest vector of `rec` reaches (h264_edge_cases.mc_pad).  The records run
+    in put-then-avg order, as the batch call promises whatever their order in `rec`."""
+    import h264_edge_cases as ec
+    pw, ph = pw or y.shape[1], ph or y.shape[0]
+    cph = ph if c422 else ph >> 1
+    pad = ec.mc_pad(rec, pw, ph)                      # (also enough for 4:2:2 chroma: its rows reach no farther than the luma taps)
+    pr = [(np.pad(r[0][:ph, :pw], pad, mode="edge"), np.pad(r[1][:cph, :pw >> 1], pad, mode="edge"), np.pad(r[2][:cph, :pw >> 1], pad, mode="edge"))
+          for r in refs]
+    rec = np.concatenate([rec[rec["avg"] == 0], rec[rec["avg"] != 0]])
     sizes = {16: 0, 8: 1, 4: 2, 2: 3}
     sb, dt = y.itemsize, y.dtype
     qpel = (lambda avg, sidx, mc, dst, src, st: o.h264_qpel(avg, sidx, mc, dst, src, st)) if bits == 8 else \
@@ -211,11 +219,34 @@ def smooth_picture422(mb_w, mb_h, bits, seed):
 
 
 # ---- weighted prediction and DC transforms at 9 / 10 bit ------------------------------------------------------------------------------------
+WIDX = {16: 0, 8: 1, 4: 2, 2: 3}
+
+
+def oracle_weight(o, bits, rec, plane, src=None):
+    """the reference's weight_h264_pixels / biweight_h264_pixels at `bits` over `rec` (byte offsets) in place on `plane`"""
+    st = plane.strides[0]
+    for r in rec:
+        if src is not None:
+            o.h264_hbd_biweight(bits, WIDX[int(r["w"])], at(plane, r["off"]), at(src, r["off"]), st, int(r["h"]), int(r["log2_denom"]), int(r["weight"]),
+                                int(r["weight_src"]), int(r["offset"]))
+        else:
+            o.h264_hbd_weight(bits, WIDX[int(r["w"])], at(plane, r["off"]), st, int(r["h"]), int(r["log2_denom"]), int(r["weight"]), int(r["offset"]))
+
+
+def oracle_dc(o, bits, c422, recs, coeffs, luma_dc):
+    """the reference's luma / chroma (4:2:2: chroma422) DC dequantisation in place on the int32 arena `coeffs` (n, 768)"""
+    for m in range(recs.shape[0]):
+        if recs["luma_qmul"][m]:
+            o.h264_hbd_dc_dequant(bits, 0, at(coeffs, m * 768 * 4), ptr(luma_dc[m].copy()), int(recs["luma_qmul"][m]))
+        for pl in range(2):
+            if recs["chroma_qmul"][m, pl]:
+                o.h264_hbd_dc_dequant(bits, 2 if c422 else 1, at(coeffs, (m * 768 + 256 * (pl + 1)) * 4), None, int(recs["chroma_qmul"][m, pl]))
+
+
 def weight_dc_cases(run_weight, run_dc, o, bits):
     """run_weight(bits, rec, plane, src | None) -> plane after ff_h264_weight_batch_hbd_cuda; run_dc(c422, recs, coeffs, luma_dc) -> coeffs after
     ff_h264_dc_dequant_batch_hbd_cuda; both against the oracle's BIT_DEPTH > 8 functions"""
     rng = np.random.default_rng(bits)
-    widx = {16: 0, 8: 1, 4: 2, 2: 3}
     for bi in (0, 1):
         plane = rng.integers(0, 1 << bits, size=(128, 256)).astype(np.uint16)
         src = rng.integers(0, 1 << bits, size=(128, 256)).astype(np.uint16)
@@ -227,13 +258,7 @@ def weight_dc_cases(run_weight, run_dc, o, bits):
                              int(rng.integers(-128, 128)), int(rng.integers(-128, 128)), 0))
         rec = np.array(recs, dtype=synth.WEIGHT_DT)
         want = plane.copy()
-        st = want.strides[0]
-        for r in rec:
-            if bi:
-                o.h264_hbd_biweight(bits, widx[int(r["w"])], at(want, r["off"]), at(src, r["off"]), st, int(r["h"]), int(r["log2_denom"]), int(r["weight"]),
-                                    int(r["weight_src"]), int(r["offset"]))
-            else:
-                o.h264_hbd_weight(bits, widx[int(r["w"])], at(want, r["off"]), st, int(r["h"]), int(r["log2_denom"]), int(r["weight"]), int(r["offset"]))
+        oracle_weight(o, bits, rec, want, src if bi else None)
         got = run_weight(bits, rec, plane.copy(), src if bi else None)
         assert not np.array_equal(want, plane) and np.array_equal(got, want), ("weight", bits, bi, np.argwhere(got != want)[:4].tolist())
     DC_DT = np.dtype([("luma_qmul", "<u4"), ("chroma_qmul", "<u4", (2,))])
@@ -246,12 +271,7 @@ def weight_dc_cases(run_weight, run_dc, o, bits):
         coeffs = rng.integers(-300 * sc, 300 * sc, size=(n, 768)).astype(np.int32)
         luma_dc = rng.integers(-2000 * sc, 2000 * sc, size=(n, 16)).astype(np.int32)
         want = coeffs.copy()
-        for m in range(n):
-            if recs["luma_qmul"][m]:
-                o.h264_hbd_dc_dequant(bits, 0, at(want, m * 768 * 4), ptr(luma_dc[m].copy()), int(recs["luma_qmul"][m]))
-            for pl in range(2):
-                if recs["chroma_qmul"][m, pl]:
-                    o.h264_hbd_dc_dequant(bits, 2 if c422 else 1, at(want, (m * 768 + 256 * (pl + 1)) * 4), None, int(recs["chroma_qmul"][m, pl]))
+        oracle_dc(o, bits, c422, recs, want, luma_dc)
         got = run_dc(c422, recs, coeffs.copy(), luma_dc)
         assert not np.array_equal(want, coeffs) and np.array_equal(got, want), ("dc", bits, c422, np.argwhere(got != want)[:4].tolist())
 

@@ -226,12 +226,16 @@ def test_deblock_refuses_unaligned_planes(gpu, lay):
 
 
 # ---- the flush point in decoder layout ----
-def flush_batch(works, pics, refs, mb_w, mb_h, lay=ec.PAD4):
+def flush_batch(works, pics, refs, mb_w, mb_h, lay=ec.PAD4, c422=0):
     """works (test_gpu_h264flush.picture_work) and their pictures stacked into one FFH264PictureWork, planes and reference planes placed
-    by `lay`: returns (work, placed pictures, the device buffers work points to)"""
+    by `lay`: returns (work, placed pictures, the device buffers work points to).  Offsets of the works are tight byte offsets, so
+    16-bit pictures (uint16 planes, int32 coefficients) and 4:2:2 ones (c422: 16 chroma rows per macroblock) stack the same way; the
+    caller sets work.bit_depth / chroma_format_idc.  A work with "deblock" = (records, 4:2:2 records or None) in place of "info" hands
+    the loop filter its records directly."""
     from libav_b200 import device
     P = len(works)
-    W, H = 16 * mb_w, 16 * mb_h
+    W, H = 16 * mb_w * pics[0][0].itemsize, 16 * mb_h
+    CH = H if c422 else H // 2
     cat = lambda planes: [np.concatenate([p[i] for p in planes]) for i in range(3)]
     d = Placed(lay, cat(pics))
     r = [Placed(lay, [np.concatenate([p] * P) for p in rp], ref=True) for rp in refs]
@@ -239,22 +243,30 @@ def flush_batch(works, pics, refs, mb_w, mb_h, lay=ec.PAD4):
     mc, res, wrec = [], [], []
     for k, w in enumerate(works):
         m = w["mc"].copy(); m["y"] += H * k; mc.append(m)
-        rr = ec.relayout_residual(w["res"], W, ls, uvls); rr["luma_off"] += H * k * ls; rr["chroma_off"] += H // 2 * k * uvls; res.append(rr)
+        rr = ec.relayout_residual(w["res"], W, ls, uvls); rr["luma_off"] += H * k * ls; rr["chroma_off"] += CH * k * uvls; res.append(rr)
         t = w["weight"].copy(); t["off"] = ec.relayout_offsets(t["off"], W, ls) + H * k * ls; wrec.append(t)
     mc, res, wrec = np.concatenate(mc), np.concatenate(res), np.concatenate(wrec)
-    infos = [w["info"] for w in works]
-    catinfo = lambda k: np.concatenate([i[k] for i in infos], axis=0)
-    keep = {k: _dev(catinfo(k)) for k in ("mb_type", "qscale", "nnz", "cbp", "slice_table", "mv0", "mv1", "ref0", "ref1")}
-    keep["sp"] = _dev(infos[0]["slice_params"]); keep["cq"] = _dev(infos[0]["chroma_qp_table"])
-    info = tables.FFH264DeblockInfo(mb_w, mb_h, P, keep["mb_type"].ptr, keep["qscale"].ptr, keep["nnz"].ptr, keep["cbp"].ptr, keep["slice_table"].ptr,
-                                    (C.c_void_p * 2)(keep["mv0"].ptr, keep["mv1"].ptr), (C.c_void_p * 2)(keep["ref0"].ptr, keep["ref1"].ptr),
-                                    keep["sp"].ptr, infos[0]["n_slices"], keep["cq"].ptr, infos[0]["cabac"], infos[0]["t8x8"])
     n = mb_w * mb_h * P
     catw = lambda k: np.concatenate([w[k] for w in works])
     dv = dict(planes=_dev(np.array([p.ptrs for p in r], np.uint64)), mc=_dev(mc), res=_dev(res), w=_dev(wrec), co=_dev(catw("coeffs")),
               nz=_dev(catw("nnzc")), dc=_dev(catw("dc")), ldc=_dev(catw("luma_dc")), intra=_dev(catw("intra")), rec=device.DevBuf(n * 104),
-              prog=device.DevBuf(4 * 2 * mb_h * P), keep=keep, info=info, refs=r)
+              prog=device.DevBuf(4 * 2 * mb_h * P), refs=r)
     work = tables.FFH264PictureWork()
+    if "info" in works[0]:
+        infos = [w["info"] for w in works]
+        catinfo = lambda k: np.concatenate([i[k] for i in infos], axis=0)
+        keep = {k: _dev(catinfo(k)) for k in ("mb_type", "qscale", "nnz", "cbp", "slice_table", "mv0", "mv1", "ref0", "ref1")}
+        keep["sp"] = _dev(infos[0]["slice_params"]); keep["cq"] = _dev(infos[0]["chroma_qp_table"])
+        info = tables.FFH264DeblockInfo(mb_w, mb_h, P, keep["mb_type"].ptr, keep["qscale"].ptr, keep["nnz"].ptr, keep["cbp"].ptr, keep["slice_table"].ptr,
+                                        (C.c_void_p * 2)(keep["mv0"].ptr, keep["mv1"].ptr), (C.c_void_p * 2)(keep["ref0"].ptr, keep["ref1"].ptr),
+                                        keep["sp"].ptr, infos[0]["n_slices"], keep["cq"].ptr, infos[0]["cabac"], infos[0]["t8x8"])
+        dv.update(keep=keep, info=info)
+        work.deblock_info = C.pointer(info)
+    else:
+        dv["rec"] = _dev(np.concatenate([w["deblock"][0] for w in works]))
+        if c422:
+            dv["ext"] = _dev(np.concatenate([w["deblock"][1] for w in works]))
+            work.deblock_chroma422 = dv["ext"].ptr
     work.mb_w, work.mb_h, work.n_pictures = mb_w, mb_h, P
     work.luma, work.cb, work.cr = d.ptrs
     work.linesize, work.uvlinesize = ls, uvls
@@ -262,7 +274,7 @@ def flush_batch(works, pics, refs, mb_w, mb_h, lay=ec.PAD4):
     work.weight[0], work.n_weight[0] = dv["w"].ptr, wrec.shape[0]
     work.coeffs, work.coeff_stride, work.nnzc = dv["co"].ptr, 768, dv["nz"].ptr
     work.dc, work.luma_dc, work.residual, work.intra = dv["dc"].ptr, dv["ldc"].ptr, dv["res"].ptr, dv["intra"].ptr
-    work.deblock_info, work.deblock_records, work.progress = C.pointer(info), dv["rec"].ptr, dv["prog"].ptr
+    work.deblock_records, work.progress = dv["rec"].ptr, dv["prog"].ptr
     return work, d, dv
 
 
