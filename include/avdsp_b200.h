@@ -217,6 +217,70 @@ size_t ff_dnxhd_encode_workspace_cuda(const FFDnxhdEncodeWork *frames /* host ar
  * misaligned out, a NULL state or out_info, and a workspace smaller than ff_dnxhd_encode_workspace_cuda returns. */
 int ff_dnxhd_encode_frames_cuda(const FFDnxhdEncodeWork *frames /* host array */, int n, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- VC-3 / DNxHD decoder (libavcodec/dnxhddec.c) -----------------------------------------------------------------------------------------
+ * Semantics:
+ *  1. Each packet decodes as a fresh decoder context decodes it.  (A reference context caches its VLCs per CID and never clears is_444, so
+ *     within one context a bit-depth or 4:4:4 change under the same CID reuses stale tables; this call has no context.)
+ *  2. Bits at and past `size` read as zero, as the reference's checked reader sees the packet's zeroed padding.  A row's reader runs to the
+ *     end of the packet, not of its coding unit (init_get_bits is given the rest of the packet), so rows of the first field may read the
+ *     second field's bytes; truncated and damaged rows decode exactly as the reference decodes them.
+ *  3. Malformed input decodes as the reference decodes it: (2 level + 1) qscale weight wraps in 32 bits, each coefficient is truncated to
+ *     int16, last_dc accumulates unclipped and is stored truncated, the "ac tex damaged" break (a run past coefficient 63) leaves the bit
+ *     position where it is and the next block starts there, and mbaff (10-bit qscale and the interlaced_mb flag) is honoured on every CID.
+ * The codebooks are not restated: `cids` / `n_cids` is the caller's CID table (the decoder's ff_dnxhd_cid_table), searched for each header's
+ * CID as ff_dnxhd_get_cid_table does.  The VLC tables are built from the entry and cached by its address, rebuilt when its checksum changes.
+ * Refusals beyond the reference's own (each -1 with a message):
+ *  - CID 0: a fresh context takes it for its cached CID and never sets cid_table (the reference dereferences NULL);
+ *  - a CID entry whose AC, DC or run codes are not a complete prefix code (the reference indexes ac_level[-1] or skips -1 bits on a missing
+ *    code), have an AC or run code longer than 16 bits or a DC code longer than 7 (the reference's one-level DC lookup cannot reach it);
+ *  - a CID entry whose AC codes need more than 24, or whose run codes need more than 32, second-level tables of the library's lookup (a
+ *    9-bit first level, 7-bit second levels; the tables are sized for shared memory, and the entries of ff_dnxhd_cid_table need at most
+ *    14 and 24), although the reference's init_vlc accepts such a code;
+ *  - a header bit depth other than the entry's bit_depth (init_vlc then reads bit_depth + 4 DC codes from an array of another length);
+ *  - an interlaced packet whose second coding unit is not itself an interlaced field header with the first unit's CID, bit depth, chroma
+ *    format and size (the reference would reallocate the frame there, or rewrite the first field with a stale cur_field);
+ *  - a scan index within 0x280 of 2^32 (the reference's bound check wraps and it reads outside the packet). */
+#define FF_DNXHD_PIX_FMT_YUV422P   4     /* AV_PIX_FMT_YUV422P */
+#define FF_DNXHD_PIX_FMT_YUV422P10 66    /* AV_PIX_FMT_YUV422P10 (little-endian) */
+#define FF_DNXHD_PIX_FMT_YUV444P10 70    /* AV_PIX_FMT_YUV444P10 (little-endian) */
+/* What the decoder sets up for a packet before get_buffer. */
+typedef struct FFDnxhdFrameInfo {
+    int cid;
+    int width, height;           /* width: the entry's (the decoder overrides the header's); height: doubled for fields, as dnxhd_decode_header
+                                  * does when the header's height matches mb_height */
+    int pix_fmt;                 /* FF_DNXHD_PIX_FMT_* */
+    int interlaced_frame, top_field_first;
+    int sar_num, sar_den;        /* av_reduce(header width, entry width, 255) when they differ, else 0 / 1 (a fresh context's) */
+    int lines;                   /* lines each plane must hold: (mb_height * 16) << interlaced_frame, the larger field's mb_height; the decoder
+                                  * writes whole macroblocks (1088 lines for 1080p) */
+} FFDnxhdFrameInfo;
+/* dnxhd_decode_header's checks for the packet (both coding units of an interlaced one) and ff_set_dimensions's, on the host; nothing is
+ * launched.  Returns 0, the AVERROR the reference returns (AVERROR_INVALIDDATA, AVERROR(ENOSYS) for an unknown CID, AVERROR(EINVAL) for a
+ * size av_image_check_size refuses), or -1 with a message for a refusal listed above.  A decoder calls it in place of dnxhd_decode_header,
+ * then ff_set_dimensions and get_buffer as now. */
+int ff_dnxhd_probe_cuda(const uint8_t *pkt /* host */, int size, const FFDnxhdCidEntry *cids, int n_cids, FFDnxhdFrameInfo *info);
+/* One packet for ff_dnxhd_decode_frames_cuda. */
+typedef struct FFDnxhdDecodeWork {
+    const uint8_t *pkt_host;     /* the packet on the host, for its headers */
+    const uint8_t *pkt;          /* the same bytes on the device */
+    int size;
+    uint8_t *data[3];            /* device planes: 8-bit samples, or 16-bit samples at 10 bit (even addresses) */
+    int linesize[3];             /* bytes between lines: positive, even at 10 bit, at least the plane's width in bytes; U and V equal (the
+                                  * reference steps through V with U's linesize) */
+    int lines[3];                /* lines each plane holds: at least FFDnxhdFrameInfo.lines */
+    int gray;                    /* AV_CODEC_FLAG_GRAY: the chroma planes are left untouched */
+} FFDnxhdDecodeWork;
+/* Bytes of device workspace ff_dnxhd_decode_frames_cuda needs for these packets (host only, nothing launched); 0 for a batch with a packet
+ * or plane the decode call refuses. */
+size_t ff_dnxhd_decode_workspace_cuda(const FFDnxhdDecodeWork *works /* host array */, int n, const FFDnxhdCidEntry *cids, int n_cids);
+/* dnxhd_decode_frame for n packets on `stream`, without synchronising: every sample the reference decoder writes is written with its value,
+ * and nothing else.  Every packet is checked (ff_dnxhd_probe_cuda's checks, then the planes) before anything is launched; -1 with a message
+ * for a packet the probe does not accept, NULL or odd planes, linesizes that are not positive, even at 10 bit and as wide as the plane, U and V
+ * linesizes that differ, planes with fewer lines than the frame needs, a NULL device packet, and a workspace smaller than
+ * ff_dnxhd_decode_workspace_cuda returns. */
+int ff_dnxhd_decode_frames_cuda(const FFDnxhdDecodeWork *works /* host array */, int n, const FFDnxhdCidEntry *cids, int n_cids, void *workspace,
+                                size_t workspace_bytes, void *stream);
+
 /* ff_xvid_idct / xvid_idct_put / xvid_idct_add (libavcodec/xvididct.c:272-331) over n blocks -- the IDCT ff_xvid_idct_init() installs for
  * MPEG-4 streams written by Xvid and for idct_algo FF_IDCT_XVID.  Arguments, addressing, mode 0 / 1 / 2 and `clear` exactly as
  * ff_simple_idct_batch_cuda; mode 2 leaves the transform result in the blocks.  Blocks at any 2-byte alignment and destinations at any

@@ -64,6 +64,9 @@ PROTOTYPES = {
     "ff_prores_encode_frames_cuda": (i32, [vp, i32, vp, sz, vp]),
     "ff_dnxhd_encode_workspace_cuda": (sz, [vp, i32]),
     "ff_dnxhd_encode_frames_cuda": (i32, [vp, i32, vp, sz, vp]),
+    "ff_dnxhd_probe_cuda": (i32, [vp, i32, vp, i32, vp]),
+    "ff_dnxhd_decode_workspace_cuda": (sz, [vp, i32, vp, i32]),
+    "ff_dnxhd_decode_frames_cuda": (i32, [vp, i32, vp, i32, vp, sz, vp]),
     "ff_xvid_idct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_faanidct_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, i32, vp]),
     "ff_pixels_clamped_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, i32, vp]),

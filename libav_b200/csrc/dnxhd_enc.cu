@@ -21,12 +21,11 @@
 //   write   one thread per macroblock: its qscale and 8 blocks at its known bit offset, ORed into the zeroed packet.
 // Except the search, threads never communicate, so the file also compiles for tests/hostsim/.
 #include "common.cuh"
+#include "dnxhd_cid.cuh"
 #include "dnxhd_enc.cuh"
 #include "../../include/avdsp_b200.h"
 #include <limits.h>
 #include <math.h>
-#include <map>
-#include <mutex>
 #include <string.h>
 #include <vector>
 
@@ -392,22 +391,6 @@ __global__ void __launch_bounds__(128) dn_write_kernel(const __grid_constant__ D
 // ---- host side ------------------------------------------------------------------------------------------------------------------------------
 int dn_refuse(const char *msg) { set_error_msg("ff_dnxhd_encode_frames_cuda", msg); return -1; }
 
-// the arrays of an entry that the tables are built from, and how many of each (dc: bit_depth + 4 codes, ac: 257, run: 62)
-uint64_t dn_checksum(const FFDnxhdCidEntry &e)
-{
-    uint64_t h = 0xcbf29ce484222325ull;
-    auto mix = [&](const void *p, size_t n) {
-        const uint8_t *b = (const uint8_t *)p;
-        for (size_t k = 0; k < n; k++) h = (h ^ b[k]) * 0x100000001b3ull;
-    };
-    mix(&e.cid, 8 * sizeof(int));
-    const size_t ndc = (size_t)e.bit_depth + 4;
-    mix(e.luma_weight, 64); mix(e.chroma_weight, 64); mix(e.dc_codes, ndc); mix(e.dc_bits, ndc);
-    mix(e.ac_codes, 257 * 2); mix(e.ac_bits, 257); mix(e.ac_level, 257); mix(e.ac_run_flag, 257); mix(e.ac_index_flag, 257);
-    mix(e.run_codes, 62 * 2); mix(e.run_bits, 62); mix(e.run, 62);
-    return h;
-}
-
 // dnxhd_init_vlc and the fixed tables on the host; -1 (with a message) for an entry the reference's asserts would reject
 int dn_build_tables(const FFDnxhdCidEntry &e, DnTables &T)
 {
@@ -458,32 +441,6 @@ int dn_build_tables(const FFDnxhdCidEntry &e, DnTables &T)
         T.aan[i] = (uint16_t)floor(16384.0 * au * av + 0.5);
     }
     return 0;
-}
-
-struct DnCached { DnTables *d; uint64_t sum; };
-std::mutex g_dn_mu;
-std::map<const FFDnxhdCidEntry *, DnCached> g_dn_tables;
-
-// the device tables of an entry: cached by its host address, rebuilt when its checksum changes (the old copy stays alive: a launch still
-// queued may read it)
-const DnTables *dn_tables_device(const FFDnxhdCidEntry *e)
-{
-    const uint64_t sum = dn_checksum(*e);
-    std::lock_guard<std::mutex> lk(g_dn_mu);
-    auto it = g_dn_tables.find(e);
-    if (it != g_dn_tables.end() && it->second.sum == sum) return it->second.d;
-    std::vector<uint8_t> host(sizeof(DnTables));
-    DnTables &T = *reinterpret_cast<DnTables *>(host.data());
-    if (dn_build_tables(*e, T)) return nullptr;
-    DnTables *d = nullptr;
-    if (cudaMalloc(&d, sizeof(DnTables)) != cudaSuccess) { set_error("ff_dnxhd_encode_frames_cuda", cudaGetLastError()); return nullptr; }
-    if (cudaMemcpy(d, &T, sizeof(DnTables), cudaMemcpyHostToDevice) != cudaSuccess) {
-        set_error("ff_dnxhd_encode_frames_cuda", cudaGetLastError());
-        cudaFree(d);
-        return nullptr;
-    }
-    g_dn_tables[e] = DnCached{ d, sum };
-    return d;
 }
 
 size_t dn_align(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -651,7 +608,7 @@ int ff_dnxhd_encode_frames_cuda(const FFDnxhdEncodeWork *frames, int n, void *wo
     }
     if (!workspace || workspace_bytes < need) return dn_refuse("workspace missing or smaller than ff_dnxhd_encode_workspace_cuda returns");
     for (int k = 0; k < n; k++)
-        if (!(tabs[k] = dn_tables_device(frames[k].cid_table))) return -1;
+        if (!(tabs[k] = dn_tables_cached<DnTables>(frames[k].cid_table, dn_build_tables, "ff_dnxhd_encode_frames_cuda"))) return -1;
     uint8_t *ws = (uint8_t *)workspace;
     for (int g0 = 0; g0 < n; g0 += DN_FRAMES_PER_LAUNCH) {
         const int m = n - g0 < DN_FRAMES_PER_LAUNCH ? n - g0 : DN_FRAMES_PER_LAUNCH;

@@ -60,6 +60,16 @@ class FFDnxhdEncodeWork(C.Structure):       # include/avdsp_b200.h
                 ("out", C.c_void_p), ("out_capacity", C.c_size_t), ("out_info", C.c_void_p)]
 
 
+class FFDnxhdFrameInfo(C.Structure):        # include/avdsp_b200.h
+    _fields_ = [("cid", C.c_int), ("width", C.c_int), ("height", C.c_int), ("pix_fmt", C.c_int), ("interlaced_frame", C.c_int),
+                ("top_field_first", C.c_int), ("sar_num", C.c_int), ("sar_den", C.c_int), ("lines", C.c_int)]
+
+
+class FFDnxhdDecodeWork(C.Structure):       # include/avdsp_b200.h
+    _fields_ = [("pkt_host", C.c_void_p), ("pkt", C.c_void_p), ("size", C.c_int), ("data", C.c_void_p * 3), ("linesize", C.c_int * 3),
+                ("lines", C.c_int * 3), ("gray", C.c_int)]
+
+
 class FDCTDSPContext(C.Structure):          # libavcodec/fdctdsp.h:26-29
     _fields_ = [("fdct", _idct), ("fdct248", _idct)]
 
