@@ -131,6 +131,67 @@ typedef struct FFProresPictureWork {
  * small for whole macroblocks (width or mb_rows), a slice count that does not cover the picture, or NULL slices / blocks. */
 int ff_prores_decode_pictures_cuda(const FFProresPictureWork *pictures /* host array */, int n, void *stream);
 
+/* ---- ProRes decoder, whole packets (libavcodec/proresdec.c: decode_frame) ---------------------------------------------------------------
+ * Semantics:
+ *  1. Each packet decodes as a fresh decoder context decodes it.  (A reference context carries nothing that changes the samples from one
+ *     packet to the next: decode_frame_header rewrites qmat_luma / qmat_chroma for every frame and decode_picture_header resets each
+ *     slice's prev_slice_sf, so this call has no context.)
+ *  2. A slice's errors never abort the frame (avctx->execute ignores decode_slice's return value).  Within a slice: a slice under 6 bytes,
+ *     or with plane sizes that do not fit it or a header size under 6, writes nothing; a plane whose AC decoding fails is not written, and
+ *     neither is any plane after it; alpha is written only when Y, U and V all decoded and the slice has alpha bytes.
+ *  3. Each slice plane is read with the reference's checked long reader: past the plane's end it sees the packet's following bytes, past
+ *     the packet's end zeros (the packet's padding); the position stops at the plane's bits + 8; get_bits_left and the MAX_PADDING test are
+ *     relative to the plane.
+ *  4. decode_vlc_codeword's exp-Golomb branch shifts by 32 - len with len up to 68 (a run of zero bits, as on a zero-filled plane, whose
+ *     DC decoding has no end guard).  A negative count is undefined in C; the reference as compiled for x86-64 shifts by the count modulo
+ *     32, and so does this call.
+ *  5. Arithmetic wraps as the compiled reference's does: DC (prev_dc, delta) and AC levels are truncated to int16, a code read as a
+ *     negative run or level ends the plane with an error, and each scaled matrix entry is (int16_t)(qmat * sf).
+ *  6. Header oddities decode as the reference decodes them: a frame header hdr_size below 20 still reads bytes 8..19; a first
+ *     pic_data_size of 0 decodes the same picture data again into the second field; a pic_data_size of 2^31 or more is an error before its
+ *     picture is decoded; a second picture header that fails leaves the first field written (FFProresFrameInfo.result).
+ * Refusals beyond the reference's own (each -1 with a message): a packet the probe does not return 0 for (no frame exists to write); a zero
+ * width or height (get_buffer refuses such a frame); NULL or odd planes; linesizes that are not even, not positive, or narrower than whole
+ * macroblocks (32 bytes per macroblock for luma, alpha and 4:4:4 chroma, 16 for 4:2:2 chroma); planes with fewer than
+ * FFProresFrameInfo.lines lines; a missing alpha plane for a format with alpha; a NULL device packet; a workspace smaller than
+ * ff_prores_decode_workspace_cuda returns, or not 16-byte aligned (its coefficient blocks are zeroed and read 16 bytes at a time). */
+#define FF_PRORES_PIX_FMT_YUV422P10  66      /* AV_PIX_FMT_YUV422P10 (little-endian) */
+#define FF_PRORES_PIX_FMT_YUV444P10  70      /* AV_PIX_FMT_YUV444P10 */
+#define FF_PRORES_PIX_FMT_YUVA422P10 92      /* AV_PIX_FMT_YUVA422P10 */
+#define FF_PRORES_PIX_FMT_YUVA444P10 94      /* AV_PIX_FMT_YUVA444P10 */
+/* What decode_frame sets up for a packet, and what it returns. */
+typedef struct FFProresFrameInfo {
+    int pix_fmt;                 /* FF_PRORES_PIX_FMT_* */
+    int interlaced_frame, top_field_first;
+    int color_primaries, color_trc, colorspace;  /* the frame header's three colour bytes */
+    int lines;                   /* lines each plane must hold: num_y_mbs * 16 << interlaced_frame (the decoder writes whole macroblocks, in
+                                  * width and in height) */
+    int pictures;                /* pictures the decoder decodes: 0, 1 or 2 (fewer than the frame's when a picture header fails) */
+    int result;                  /* decode_frame's return value: the packet size, or AVERROR_INVALIDDATA after a failing picture header */
+} FFProresFrameInfo;
+/* decode_frame's checks up to get_buffer (the frame atom, decode_frame_header) on the host, and both decode_picture_header calls' (the
+ * slice-table sums included); nothing is launched.  width / height: the caller's avctx dimensions, which the header must match.  Returns
+ * 0, the AVERROR_INVALIDDATA the reference returns before get_buffer, or -1 with a message for a refusal listed above.  A decoder calls it
+ * in place of decode_frame_header, then get_buffer, then ff_prores_decode_frames_cuda, and returns info.result. */
+int ff_prores_probe_cuda(const uint8_t *pkt_host, int size, int width, int height, FFProresFrameInfo *info);
+/* One packet for ff_prores_decode_frames_cuda. */
+typedef struct FFProresDecodeWork {
+    const uint8_t *pkt_host;     /* the packet on the host, for its headers */
+    const uint8_t *pkt;          /* the same bytes on the device */
+    int size;
+    int width, height;           /* avctx->width / height */
+    uint8_t *data[4];            /* device planes of 16-bit samples (even addresses): y, u, v, and alpha for the yuva formats */
+    int linesize[4];             /* bytes between the frame's lines: even, positive, at least the width of whole macroblocks */
+    int lines[4];                /* lines each plane holds: at least FFProresFrameInfo.lines */
+} FFProresDecodeWork;
+/* Bytes of device workspace ff_prores_decode_frames_cuda needs for these packets (host only, nothing launched); 0 for a batch with a packet
+ * or plane the decode call refuses. */
+size_t ff_prores_decode_workspace_cuda(const FFProresDecodeWork *works /* host array */, int n);
+/* decode_frame for n packets on `stream`, without synchronising: every sample the reference decoder writes is written with its value (the
+ * alpha plane, and the pictures before a failing second picture header, included), and nothing else.  Every packet is checked (the probe's
+ * checks, then the planes) before anything is launched; -1 with a message for a refusal listed above. */
+int ff_prores_decode_frames_cuda(const FFProresDecodeWork *works /* host array */, int n, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- ProRes encoder (libavcodec/proresenc.c) --------------------------------------------------------------------------------------------
  * One frame for ff_prores_encode_frames_cuda: the source planes and the encoder's options, as encode_init / encode_frame take them. */
 typedef struct FFProresEncodeWork {

@@ -60,6 +60,9 @@ PROTOTYPES = {
     "ff_simple_idct10_batch_cuda": (i32, [i32, vp, vp, vp, pd, sz, vp]),
     "ff_prores_idct_put_batch_cuda": (i32, [vp, vp, vp, pd, vp, vp, sz, vp]),
     "ff_prores_decode_pictures_cuda": (i32, [vp, i32, vp]),
+    "ff_prores_probe_cuda": (i32, [vp, i32, i32, i32, vp]),
+    "ff_prores_decode_workspace_cuda": (sz, [vp, i32]),
+    "ff_prores_decode_frames_cuda": (i32, [vp, i32, vp, sz, vp]),
     "ff_prores_encode_workspace_cuda": (sz, [vp, i32]),
     "ff_prores_encode_frames_cuda": (i32, [vp, i32, vp, sz, vp]),
     "ff_dnxhd_encode_workspace_cuda": (sz, [vp, i32]),

@@ -16,6 +16,7 @@
   oracle/_ref/libproresencref.so TEST ONLY: the reference's ProRes encoder with every option and its tables, same conditions
   oracle/_ref/libdnxhdencref.so TEST ONLY: the reference's VC-3 / DNxHD encoder with every option and its CID tables, same conditions
   oracle/_ref/libdnxhddecref.so TEST ONLY: the reference's VC-3 / DNxHD decoder and its CID table, same conditions
+  oracle/_ref/libproresdecref.so TEST ONLY: the reference's ProRes decoder with the checked bitstream reader, same conditions
 All outputs are in-tree so they travel to the GPU box with the snapshot.
 """
 import glob
@@ -91,7 +92,8 @@ def build_oracle_ref(force=False):
     """Compile the reference's own C sources (read in place) with oracle/refbuild/Makefile: libavref.so, its timing-only SIMD
     flavour and the satellite libraries of single features, all in one make run; then the S-VOP library with mpvgmc.mk and
     the any-chroma-format MPEG-2 library with mpvcf.mk, the FAAN encoder libraries with faan.mk and the ProRes libraries with
-    prores.mk and prores_enc.mk and the DNxHD encoder and decoder libraries with dnxhd_enc.mk and dnxhd_dec.mk, which take their rules from that Makefile."""
+    prores.mk, prores_enc.mk and prores_dec.mk and the DNxHD encoder and decoder libraries with dnxhd_enc.mk and dnxhd_dec.mk, which
+    take their rules from that Makefile."""
     if not os.path.isdir(REFERENCE):
         return ORACLE_REF if os.path.exists(ORACLE_REF) else None
     if force:
@@ -102,6 +104,7 @@ def build_oracle_ref(force=False):
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "faan.mk", "REF=" + REFERENCE])
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "prores.mk", "REF=" + REFERENCE])
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "prores_enc.mk", "REF=" + REFERENCE])
+    _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "prores_dec.mk", "REF=" + REFERENCE])
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "dnxhd_enc.mk", "REF=" + REFERENCE])
     _run(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "refbuild"), "-f", "dnxhd_dec.mk", "REF=" + REFERENCE])
     return ORACLE_REF

@@ -15,7 +15,7 @@
 #ifndef AVB_HOSTSIM
 #include "block_stage.cuh"
 #endif
-#include "../../include/avdsp_b200.h"
+#include "prores.cuh"
 #include <string.h>
 
 namespace avb {
@@ -43,17 +43,16 @@ struct PrPic {
     size_t n_blocks;
     uint8_t qm[2][64];
 };
-struct PrLaunch { PrPic pic[PR_PICS_PER_LAUNCH]; };
+// ST: the whole-packet decoder's launch (prores_dec.cu), which adds per picture its slices' plane status (prores.cuh)
+template <bool ST> struct PrLaunch { PrPic pic[PR_PICS_PER_LAUNCH]; };
+template <> struct PrLaunch<true> { PrPic pic[PR_PICS_PER_LAUNCH]; const uint32_t *status[PR_PICS_PER_LAUNCH]; };
+__device__ __forceinline__ const uint32_t *pr_status(const PrLaunch<false> &, int) { return nullptr; }
+__device__ __forceinline__ const uint32_t *pr_status(const PrLaunch<true> &L, int k) { return L.status[k]; }
 
-// decode_picture's slice grid: 1 << swf macroblocks per slice, the width halving at the right edge until the slice fits
-__host__ __device__ inline int pr_slices_per_row(int mb_w, int swf)
-{
-    const int rem = mb_w & ((1 << swf) - 1);
-    return (mb_w >> swf) + (rem & 1) + ((rem >> 1) & 1) + ((rem >> 2) & 1);
-}
-
-// block i of a picture's coefficient buffer -> its destination and which matrix / scale factor dequantise it; false: no slice holds it
-__device__ __forceinline__ bool pr_locate(const PrPic &P, size_t i, uint8_t *&dst, ptrdiff_t &ls, int &chroma, int &sf)
+// block i of a picture's coefficient buffer -> its destination and which matrix / scale factor dequantise it; false: no slice holds it, or
+// (ST) its slice does not write its plane
+template <bool ST>
+__device__ __forceinline__ bool pr_locate(const PrPic &P, const uint32_t *status, size_t i, uint8_t *&dst, ptrdiff_t &ls, int &chroma, int &sf)
 {
     // The decoder stages its slices back to back in slice order, so block i's slice follows from the geometry; one load confirms it.
     // Any other table takes a binary search for the last slice whose first block is <= i.
@@ -105,6 +104,7 @@ __device__ __forceinline__ bool pr_locate(const PrPic &P, size_t i, uint8_t *&ds
         if (P.c444) { dx = (pos >> 1) * 8; dy = (pos & 1) * 8; mbw = 16; }   // TL, BL, TR, BR
         else        { dx = 0; dy = pos * 8; mbw = 8; }                       // top, bottom
     }
+    if (ST && !pr_plane_written(status[lo], p)) return false;
     ls = P.ls[p];
     dst = P.plane[p] + (ptrdiff_t)(sy * 16 + dy) * ls + (ptrdiff_t)(((x + mb) * mbw + dx) * 2);
     chroma = p != 0;
@@ -172,13 +172,14 @@ __global__ void __launch_bounds__(128) prores_idct_block_kernel(const PrBatch B)
     pr_store_samples(B.frame + B.dst_off[i], B.stride, o);
 }
 
-__global__ void __launch_bounds__(128) prores_picture_block_kernel(const __grid_constant__ PrLaunch L)
+template <bool ST>
+__global__ void __launch_bounds__(128) prores_picture_block_kernel(const __grid_constant__ PrLaunch<ST> L)
 {
     const PrPic &P = L.pic[blockIdx.y];
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.n_blocks) return;
     uint8_t *dst; ptrdiff_t ls; int chroma, sf;
-    if (!pr_locate(P, i, dst, ls, chroma, sf)) return;
+    if (!pr_locate<ST>(P, pr_status(L, blockIdx.y), i, dst, ls, chroma, sf)) return;
     const int16_t *g = P.blocks + 64 * i;
     uint4 row[8];
     for (int r = 0; r < 8; r++) row[r] = pr_dequant(pr_load_row(g, r), pr_qrow(P.qm[chroma] + 8 * r, sf));
@@ -194,8 +195,9 @@ __global__ void __launch_bounds__(128) prores_picture_block_kernel(const __grid_
 // samples leave as eight 16-byte rows per lane: 384 B per block.  Picture (PIC true, one picture per blockIdx.y): each lane derives its
 // block's destination and matrix, before it waits for the group's coefficients so that the slice search overlaps their arrival; nothing
 // goes back to the coefficients: 256 B per block.
-template <bool PIC>
-__device__ __forceinline__ void pr_staged(const PrBatch *B, const PrPic *P, uint4 (&tile)[PR_WARPS][2][256], const uint8_t (*qm)[64])
+template <bool PIC, bool ST = false>
+__device__ __forceinline__ void pr_staged(const PrBatch *B, const PrPic *P, uint4 (&tile)[PR_WARPS][2][256], const uint8_t (*qm)[64],
+                                          const uint32_t *status = nullptr)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int16_t *blocks = PIC ? const_cast<int16_t *>(P->blocks) : B->blocks;
@@ -215,7 +217,7 @@ __device__ __forceinline__ void pr_staged(const PrBatch *B, const PrPic *P, uint
         ptrdiff_t ls = PIC ? 0 : B->stride;
         int chroma = 0, sf = 0;
         const uint4 *q = nullptr;
-        if (PIC) live = live && pr_locate(*P, i, dst, ls, chroma, sf);
+        if (PIC) live = live && pr_locate<ST>(*P, status, i, dst, ls, chroma, sf);
         else {
             q = reinterpret_cast<const uint4 *>(B->qmats + 64 * (size_t)(live && B->qidx ? B->qidx[i] : 0));
             if (live) dst = B->frame + B->dst_off[i];
@@ -249,14 +251,15 @@ __global__ void __launch_bounds__(PR_WARPS * 32) prores_idct_staged_kernel(const
     pr_staged<false>(&B, nullptr, tile, nullptr);
 }
 
-__global__ void __launch_bounds__(PR_WARPS * 32) prores_picture_staged_kernel(const __grid_constant__ PrLaunch L)
+template <bool ST>
+__global__ void __launch_bounds__(PR_WARPS * 32) prores_picture_staged_kernel(const __grid_constant__ PrLaunch<ST> L)
 {
     __shared__ __align__(128) uint4 tile[PR_WARPS][2][256];
     __shared__ __align__(16) uint8_t qm[2][64];
     const PrPic &P = L.pic[blockIdx.y];
     qm[threadIdx.x >> 6][threadIdx.x & 63] = P.qm[threadIdx.x >> 6][threadIdx.x & 63];
     __syncthreads();
-    pr_staged<true>(nullptr, &P, tile, qm);
+    pr_staged<true, ST>(nullptr, &P, tile, qm, pr_status(L, blockIdx.y));
 }
 
 // resident CTAs of a staged kernel over the whole device: the persistent grids never exceed one wave
@@ -283,6 +286,9 @@ int launch_prores_batch(const PrBatch &B, cudaStream_t st)
     AVB_LAUNCH(prores_idct_block_kernel, dim3((unsigned)((B.n + 127) / 128)), dim3(128), 0, st)(B);
     return check_launch("ff_prores_idct_put_batch_cuda");
 }
+
+void pr_set_status(PrLaunch<false> &, int, const uint32_t *const *, int) {}
+void pr_set_status(PrLaunch<true> &L, int k, const uint32_t *const *status, int i) { L.status[k] = status[i]; }
 
 int pr_refuse(const char *msg) { set_error_msg("ff_prores_decode_pictures_cuda", msg); return -1; }
 
@@ -311,11 +317,12 @@ int pr_picture(const FFProresPictureWork &w, PrPic &P)
 }
 
 // pictures already checked by pr_picture; up to PR_PICS_PER_LAUNCH per launch, each picture one row (blockIdx.y) of the grid
-int launch_prores_pictures(const FFProresPictureWork *pictures, int n, cudaStream_t st)
+template <bool ST>
+int launch_pictures(const FFProresPictureWork *pictures, const uint32_t *const *status, int n, cudaStream_t st)
 {
     for (int g0 = 0; g0 < n; g0 += PR_PICS_PER_LAUNCH) {
         const int m = n - g0 < PR_PICS_PER_LAUNCH ? n - g0 : PR_PICS_PER_LAUNCH;
-        PrLaunch L;
+        PrLaunch<ST> L;
         memset(&L, 0, sizeof(L));
         size_t most = 0;
         bool aligned = true;
@@ -323,19 +330,20 @@ int launch_prores_pictures(const FFProresPictureWork *pictures, int n, cudaStrea
             pr_picture(pictures[g0 + k], L.pic[k]);
             most = L.pic[k].n_blocks > most ? L.pic[k].n_blocks : most;
             aligned = aligned && !((uintptr_t)L.pic[k].blocks & 15);
+            pr_set_status(L, k, status, g0 + k);
         }
         if (!most) continue;
 #ifndef AVB_HOSTSIM
         if (aligned) {
-            static const unsigned wave = pr_wave(prores_picture_staged_kernel);
+            static const unsigned wave = pr_wave(prores_picture_staged_kernel<ST>);
             const size_t groups = (most + 31) / 32;
             const unsigned grid = (unsigned)max((size_t)1, min((size_t)(wave / (unsigned)m), (groups + PR_WARPS - 1) / PR_WARPS));
-            prores_picture_staged_kernel<<<dim3(grid, m), PR_WARPS * 32, 0, st>>>(L);
+            prores_picture_staged_kernel<ST><<<dim3(grid, m), PR_WARPS * 32, 0, st>>>(L);
             if (check_launch("ff_prores_decode_pictures_cuda")) return -1;
             continue;
         }
 #endif
-        AVB_LAUNCH(prores_picture_block_kernel, dim3((unsigned)((most + 127) / 128), m), dim3(128), 0, st)(L);
+        AVB_LAUNCH(prores_picture_block_kernel<ST>, dim3((unsigned)((most + 127) / 128), m), dim3(128), 0, st)(L);
         if (check_launch("ff_prores_decode_pictures_cuda")) return -1;
     }
     return 0;
@@ -366,6 +374,12 @@ void slot_prores_idct_put(uint16_t *out, ptrdiff_t linesize, int16_t *block, con
 }
 
 }  // namespace
+
+int launch_prores_pictures(const FFProresPictureWork *pictures, int n, cudaStream_t st, const uint32_t *const *status)
+{
+    return status ? launch_pictures<true>(pictures, status, n, st) : launch_pictures<false>(pictures, nullptr, n, st);
+}
+
 }  // namespace avb
 
 using namespace avb;

@@ -33,6 +33,16 @@ class FFProresPictureWork(C.Structure):     # include/avdsp_b200.h
                 ("blocks", C.c_void_p), ("n_blocks", C.c_size_t)]
 
 
+class FFProresFrameInfo(C.Structure):       # include/avdsp_b200.h
+    _fields_ = [("pix_fmt", C.c_int), ("interlaced_frame", C.c_int), ("top_field_first", C.c_int), ("color_primaries", C.c_int),
+                ("color_trc", C.c_int), ("colorspace", C.c_int), ("lines", C.c_int), ("pictures", C.c_int), ("result", C.c_int)]
+
+
+class FFProresDecodeWork(C.Structure):      # include/avdsp_b200.h
+    _fields_ = [("pkt_host", C.c_void_p), ("pkt", C.c_void_p), ("size", C.c_int), ("width", C.c_int), ("height", C.c_int),
+                ("data", C.c_void_p * 4), ("linesize", C.c_int * 4), ("lines", C.c_int * 4)]
+
+
 class FFProresEncodeWork(C.Structure):      # include/avdsp_b200.h
     _fields_ = [("data", C.c_void_p * 4), ("linesize", C.c_int * 4), ("width", C.c_int), ("height", C.c_int), ("pix_fmt", C.c_int),
                 ("interlaced", C.c_int), ("profile", C.c_int), ("mbs_per_slice", C.c_int), ("bits_per_mb", C.c_int),
